@@ -105,11 +105,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Bounded wait: a protocol bug traps (=> launch error reported to the host) instead of hanging the GPU.
+// No printf on the timeout path: it compiles to a call, and ptxas serialises every wgmma of a mainloop that can reach a call
+// (C7510).  Build with -DDSB_MBAR_DEBUG to print the waiting block / thread before the trap, at that cost.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if (++spins > (1u << 26)) {
+#ifdef DSB_MBAR_DEBUG
       printf("dsb: mbarrier wait timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
+#endif
       __trap();
     }
   }

@@ -18,6 +18,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cstdlib>
+#include <type_traits>
 
 namespace dsb {
 
@@ -75,7 +76,8 @@ struct GemmSmem {
 
 // One 16-row x 32-column chunk of the output tile for one warp: the chunk sits in `sw` (XOR-swizzled float4 groups, row stride 32 floats);
 // alpha / bias / residual / activation / rounding / border mask, then coalesced stores (lanes 0-7 cover one row's 32 columns).
-__device__ __noinline__ void epilogue_chunk(const GemmParams& p, const float* sw, int row_base, int col0, int b, int lane, bool vec_ok) {
+// Inlined: the call (one per chunk) and its ABI register traffic cost the split-fp16 denoiser GEMMs 4-10 % of their time on an H100.
+__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const float* sw, int row_base, int col0, int b, int lane, bool vec_ok) {
   const bool has_geo = p.geo_P > 0;
   const int out_mode = (p.flags & DSB_GEMM_OUT_F16_SPLIT) ? 3 : ((p.flags & DSB_GEMM_OUT_F16) ? 1 : ((p.flags & DSB_GEMM_OUT_BF16) ? 2 : 0));
   const int act = (p.flags & DSB_GEMM_GELU2) ? 1 : ((p.flags & DSB_GEMM_LRELU) ? 2 : ((p.flags & DSB_GEMM_TANH) ? 3 : 0));
@@ -380,7 +382,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       int prev_stage = -1;
       if constexpr (F3) {
         // parity-grade form: the wgmma accumulator does not round every addition like an fp32 FADD, which over K = 4096 costs more than
-        // the 22-bit operands allow; each k-block's 3 x 64-deep partial sum is therefore promoted into the fp32 accumulator with FADDs
+        // the 22-bit operands allow; each k-block's 3 x 64-deep partial sum is therefore promoted into the fp32 accumulator with FADDs.
+        // The pipe drains once per k-block for this.  Overlapping the promotion with the next k-block (two partial accumulators,
+        // wgmma_wait<1>) measured slower on an H100, see DESIGN section 4.
         float part[64];
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&full_bar[stage], phase);
@@ -397,28 +401,34 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           for (int i = 0; i < 64; ++i) acc[0][i] += part[i];
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-      } else for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_u32(smem + stage * S::STAGE_BYTES);
+      } else {
+        // the MN-major choice is made once per tile, outside the wgmma window: a branch between wgmma_fence and commit makes
+        // ptxas inject warpgroup.arrive (C7519) around every MMA
+        auto mainloop = [&](auto ta, auto tb) {
+          for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t sa = smem_u32(smem + stage * S::STAGE_BYTES);
 #pragma unroll
-        for (int h = 0; h < NH; ++h) wgmma_fence_regs(acc[h]);
-        wgmma_fence();
-        if constexpr (KIND == DSB_DTYPE_TF32 || F3) {
-          mma_kblock<KIND, 0, 0, NH, false>(acc, sa, wg, kb);
-        } else {
-          if (!p.a_mn && !p.b_mn) mma_kblock<KIND, 0, 0, NH, false>(acc, sa, wg, kb);
-          else if (p.a_mn && !p.b_mn) mma_kblock<KIND, 1, 0, NH, false>(acc, sa, wg, kb);
-          else if (!p.a_mn) mma_kblock<KIND, 0, 1, NH, false>(acc, sa, wg, kb);
-          else mma_kblock<KIND, 1, 1, NH, false>(acc, sa, wg, kb);
-        }
-        wgmma_commit();
+            for (int h = 0; h < NH; ++h) wgmma_fence_regs(acc[h]);
+            wgmma_fence();
+            mma_kblock<KIND, decltype(ta)::value, decltype(tb)::value, NH, false>(acc, sa, wg, kb);
+            wgmma_commit();
 #pragma unroll
-        for (int h = 0; h < NH; ++h) wgmma_fence_regs(acc[h]);
-        // keep one k-block of MMAs in flight: the previous one has retired, so its smem slot goes back to the producer
-        wgmma_wait<1>();
-        if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-        prev_stage = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            for (int h = 0; h < NH; ++h) wgmma_fence_regs(acc[h]);
+            // keep one k-block of MMAs in flight: the previous one has retired, so its smem slot goes back to the producer
+            wgmma_wait<1>();
+            if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+            prev_stage = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          }
+        };
+        using K0 = std::integral_constant<int, 0>;
+        using K1 = std::integral_constant<int, 1>;
+        if constexpr (KIND == DSB_DTYPE_TF32) mainloop(K0{}, K0{});
+        else if (!p.a_mn && !p.b_mn) mainloop(K0{}, K0{});
+        else if (p.a_mn && !p.b_mn) mainloop(K1{}, K0{});
+        else if (!p.a_mn) mainloop(K0{}, K1{});
+        else mainloop(K1{}, K1{});
       }
       wgmma_wait<0>();
 #pragma unroll
