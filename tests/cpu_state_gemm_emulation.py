@@ -120,9 +120,9 @@ def gemm_desc(*, A, W, out, M, N, K, taps, lda, ldw, ldo, dtype=F16, batch=1, a_
             pp = rows % gP
             yy, xx = pp // gW, pp % gW
             inside = (yy >= y0) & (yy < y1) & (xx >= x0) & (xx < x1)
-            y = y * inside[:, None]
-        if amax_out is not None:
-            amax_out.fill_(max(float(amax_out), float(y.float().abs().max())))
+            y = torch.where(inside[:, None], y, 0.0)  # masked rows are stored as zeros, even where the value is inf or NaN
+        if amax_out is not None:  # torch.maximum keeps a NaN, as the kernel's integer max over |x| bit patterns does
+            amax_out.fill_(torch.maximum(amax_out.reshape(()), y.float().abs().max()))
         if flags & NO_STORE:
             continue
         base = b * out_batch_stride

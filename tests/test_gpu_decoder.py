@@ -30,9 +30,13 @@ def build_vq(K, E, ch, ch_mult, sd=None, z_channels=None, prefix="content_codec.
     return m.cuda().eval()
 
 
+# f16x3 (the default) is held to 4x the 5.0e-6 measured on an H100, far inside its north-star 1e-3
+_MEASURED_BOUND = {"f16x3": 2e-5}
+
+
 @pytest.mark.parametrize("precision,tol", [("f16x3", 1e-3), ("tf32x3", 1e-3), ("tf32", 1.5e-2)])
 def test_decoder_tiny_matches_reference_golden(G, precision, tol):
-    """north_star tolerance (1e-3 relative) holds in the default split-TF32 mode; single-pass TF32 is the fast, looser mode."""
+    """tol is the north-star tolerance (1e-3 relative) of the split modes; single-pass TF32 is the fast, looser mode."""
     sd, g = load_golden("decoder_tiny.npz")
     K, E, ch, H, W = [int(v) for v in g["__cfg"]]
     m = build_vq(K, E, ch, (1, 1, 1, 1, 2), sd, precision=precision)
@@ -41,7 +45,7 @@ def test_decoder_tiny_matches_reference_golden(G, precision, tol):
     assert mel.shape == ref.shape
     err = rel_err(mel, ref)
     print(f"decoder tiny [{precision}] rel err", err)
-    assert err < tol
+    assert err < min(tol, _MEASURED_BOUND.get(precision, tol))
     # the reference-shaped entry point (NCHW latents) agrees with the token fast path
     ids_rm = O.column_major_reverse(torch.from_numpy(g["in_ids"]).long(), H, W)
     z = O.codebook_lookup(sd, ids_rm, (ids_rm.shape[0], H, W, E))
@@ -60,7 +64,7 @@ def test_decoder_full_config_matches_oracle(G):
     err = rel_err(mel, ref)
     mse = float(((mel - ref) ** 2).mean())
     print("decoder full [default precision] rel err", err, "mel MSE", mse, "ref rms", float(ref.pow(2).mean().sqrt()))
-    assert err < 1e-3
+    assert err < 1.2e-4  # 4x the 3.1e-5 measured on an H100 in the default f16x3 mode; the north-star bound for the decoder is 1e-3
 
 
 def test_melgan_tiny_matches_reference_golden(G):

@@ -106,28 +106,60 @@ def test_gemm_epilogues_and_persistence(G):
     assert torch.equal(out.cpu(), G.tf32_round_ref(G.ops.gemm(a.cuda(), w.cuda(), bias.cuda()).cpu()))
 
 
+def _out_view(M, N, pad, dtype):
+    """A sentinel-filled (M, N + pad) buffer and its (M, N) view: the GEMM writes the view with ldo = N + pad."""
+    buf = torch.full((M, N + pad), 7.0, dtype=dtype, device="cuda")
+    return buf, buf[:, :N]
+
+
+def _residual_view(M, N, pad, g):
+    """None, or an (M, N) residual view of an (M, N + pad) buffer: ld_res = N + pad."""
+    return None if pad is None else torch.randn(M, N + pad, generator=g).cuda()[:, :N]
+
+
+def _assert_rounded(out, ref, u):
+    """Every element within the output type's rounding (u: half an ulp, relative) of the fp64 value, on top of the fp32 result's own 2e-5."""
+    ref = ref.double().cpu()
+    err = (out.double().cpu() - ref).abs()
+    assert bool((err <= u * ref.abs() + 2e-5 * float(ref.abs().max())).all())
+
+
+def _check_2byte_gemm(G, dt, M, N, K, ldo_pad=0, res_pad=None):
+    """A bf16 GEMM (no bias) or an f16 GEMM (bias + GELU2) with fp32 and 2-byte outputs, vs fp64: the fp32 output within 2e-5, the 2-byte output
+    within its type's rounding of the fp64 value, and columns beyond N of a wider output row untouched."""
+    f16 = dt == "f16"
+    g = torch.Generator().manual_seed(3 if f16 else 2)
+    a = torch.randn(M, K, generator=g).to(torch.float16 if f16 else torch.bfloat16)
+    w = (torch.randn(N, K, generator=g) * 0.05).to(a.dtype)
+    bias = torch.randn(N, generator=g) if f16 else None
+    res = _residual_view(M, N, res_pad, g)
+    ref = _ref(a.float(), w.float(), bias, None if res is None else res.cpu(), gelu=f16)
+    kw = dict(dtype=G.ops.F16 if f16 else G.ops.BF16, gelu=f16)
+    bc = None if bias is None else bias.cuda()
+    buf, out = _out_view(M, N, ldo_pad, torch.float32)
+    G.ops.gemm(a.cuda(), w.cuda(), bc, res, out=out, **kw)
+    assert G.relerr(out, ref) < 2e-5
+    bufh, outh = _out_view(M, N, ldo_pad, a.dtype)
+    G.ops.gemm(a.cuda(), w.cuda(), bc, res, out=outh, **kw)
+    assert outh.dtype == a.dtype and G.relerr(outh.float(), ref) < (1e-3 if f16 else 5e-3)
+    _assert_rounded(outh, ref, 2.0 ** (-11 if f16 else -8))
+    for b in (buf, bufh):
+        assert torch.equal(b[:, N:], torch.full_like(b[:, N:], 7.0))
+
+
 def test_gemm_bf16(G):
-    g = torch.Generator().manual_seed(2)
-    M, N, K = 777, 512, 1024
-    a = torch.randn(M, K, generator=g).bfloat16()
-    w = (torch.randn(N, K, generator=g) * 0.05).bfloat16()
-    out = G.ops.gemm(a.cuda(), w.cuda(), dtype=G.ops.BF16)
-    assert G.relerr(out, _ref(a.float(), w.float())) < 2e-5
-    outh = G.ops.gemm(a.cuda(), w.cuda(), dtype=G.ops.BF16, out_bf16=True)
-    assert G.relerr(outh.float(), _ref(a.float(), w.float())) < 5e-3
+    _check_2byte_gemm(G, "bf16", 777, 512, 1024)
 
 
 def test_gemm_f16(G):
-    g = torch.Generator().manual_seed(3)
-    M, N, K = 4240, 1024, 1024
-    a = torch.randn(M, K, generator=g).half()
-    w = (torch.randn(N, K, generator=g) * 0.05).half()
-    bias = torch.randn(N, generator=g)
-    ref = _ref(a.float(), w.float(), bias, gelu=True)
-    out = G.ops.gemm(a.cuda(), w.cuda(), bias.cuda(), dtype=G.ops.F16, gelu=True)
-    assert G.relerr(out, ref) < 2e-5
-    outh = G.ops.gemm(a.cuda(), w.cuda(), bias.cuda(), dtype=G.ops.F16, gelu=True, out_f16=True)
-    assert outh.dtype == torch.float16 and G.relerr(outh.float(), ref) < 1e-3
+    _check_2byte_gemm(G, "f16", 4240, 1024, 1024)
+
+
+# the layouts that take the scalar epilogue: an N tail (33, 100), an output view with ldo = N + 2, a residual view with ld_res = N + 1
+@pytest.mark.parametrize("M,N,K,ldo_pad,res_pad", [(300, 33, 128, 0, None), (300, 100, 256, 0, None), (300, 128, 128, 2, None), (300, 128, 128, 0, 1)])
+@pytest.mark.parametrize("dt", ["bf16", "f16"])
+def test_gemm_2byte_scalar_epilogue(G, dt, M, N, K, ldo_pad, res_pad):
+    _check_2byte_gemm(G, dt, M, N, K, ldo_pad, res_pad)
 
 
 def test_gemm_activation_flags(G):

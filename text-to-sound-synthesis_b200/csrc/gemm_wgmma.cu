@@ -148,11 +148,14 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const float*
         if (!((in_mask >> i) & 1u)) { x[4 * i] = 0.f; x[4 * i + 1] = 0.f; x[4 * i + 2] = 0.f; x[4 * i + 3] = 0.f; }
     }
     if (p.amax_out) {  // calibration runs only: largest magnitude this launch would store
-      float m = 0.f;
+      // integer max over the bit patterns of |x|: non-negative floats order like their bits and a NaN (sign cleared by fabsf) sorts above
+      // +inf, so a NaN survives into amax_out exactly as in the scalar path's atomicMax (fmaxf would drop it and calibration would pass)
+      int mi = 0;
 #pragma unroll
       for (int i = 0; i < NI; ++i)
-        if ((ok_mask >> i) & 1u) m = fmaxf(m, fmaxf(fmaxf(fabsf(x[4 * i]), fabsf(x[4 * i + 1])), fmaxf(fabsf(x[4 * i + 2]), fabsf(x[4 * i + 3]))));
-      int mi = __float_as_int(m);  // non-negative floats (and +inf, NaN payloads) order like their bit patterns
+        if ((ok_mask >> i) & 1u)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) mi = max(mi, __float_as_int(fabsf(x[4 * i + e])));
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) mi = max(mi, __shfl_xor_sync(0xffffffffu, mi, o));
       if (lane == 0) atomicMax(reinterpret_cast<int*>(p.amax_out), mi);
