@@ -33,6 +33,12 @@ def sampler_case_inputs(case, B=2, K=256, L=265):
     return logits, x_t, t, u
 
 
+def build_dt(K, D, NL, NH, CD, sd=None, spatial=(5, 53), T=100, precision="f16"):
+    """The drop-in DiffusionTransformer (the package must already be loaded)."""
+    from diffsound_b200.utils.builders import build_diffusion_transformer
+    return build_diffusion_transformer(K, D, NL, NH, CD, sd, spatial=spatial, T=T, precision=precision)
+
+
 def rel_err(a, b):
     """max |a-b| / max|b|  -- the 'relative' of north_star's 1e-3 (relative to the tensor's scale)."""
     return float((a.double() - b.double()).abs().max() / b.double().abs().max().clamp_min(1e-30))

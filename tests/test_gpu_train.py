@@ -10,8 +10,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from oracle import diffsound_oracle as O  # noqa: E402
-from tests.helpers import load_golden, portable_uniform  # noqa: E402
-from tests.test_gpu_transformer import build_dt  # noqa: E402
+from tests.helpers import build_dt, load_golden, portable_uniform  # noqa: E402
 
 SCHED_ROWS = ["log_at", "log_bt", "log_ct", "log_1_min_ct", "log_cumprod_at", "log_cumprod_bt", "log_cumprod_ct", "log_1_min_cumprod_ct"]
 
@@ -158,7 +157,8 @@ def test_embedding_backward_and_row_gather_scatter(G, TO):
     assert G.relerr(dxs, x.grad) < 1e-5
 
 
-@pytest.mark.parametrize("K", [32, 256, 512])
+# K + 1 on both sides of every register-tile boundary of train_loss_kernel<NJ> (NJ = 2, 5, 9, 17, 33 columns of 32 classes per lane)
+@pytest.mark.parametrize("K", [32, 63, 64, 159, 160, 256, 287, 288, 512, 543, 544, 1055])
 def test_q_sample_and_fused_loss_match_oracle(G, TO, K):
     """q_sample ids bit-exact vs the oracle (same uniforms); loss terms, log_model_prob and d loss/d logits vs torch autograd through the oracle."""
     B, L, T = 5, 265, 100
@@ -198,10 +198,11 @@ def test_q_sample_and_fused_loss_match_oracle(G, TO, K):
 
 
 # ------------------------------------------------------------------------------------------------ whole model
-def _grad_report(tag, grads, ref_of, tol):
+def _grad_report(tag, grads, ref_of, tol, loose=None):
     """Per-parameter max-abs error relative to that parameter's reference gradient scale.  Parameters whose true gradient is zero
     (attention key biases: softmax is invariant to a shift common to all keys) only carry rounding noise in the reference, so the scale
-    is floored at 1e-4 of the largest gradient in the model."""
+    is floored at 1e-4 of the largest gradient in the model.  loose = [(name fragments, tolerance), ...]: a parameter whose name contains one
+    of a group's fragments is held to the first such group's tolerance instead of tol.  Returns the worst error."""
     refs = {n: ref_of(n) for n in grads}
     gmax = max(float(r.abs().max()) for r in refs.values())
     rows = []
@@ -213,23 +214,25 @@ def _grad_report(tag, grads, ref_of, tol):
     rows.sort(reverse=True)
     for e, n, rm, ae in rows[:6]:
         print(f"[{tag}] {n}: rel {e:.3e} (ref max {rm:.3e}, abs err {ae:.3e})")
-    assert rows[0][0] < tol, rows[0]
+    if tol is not None:
+        for e, n, rm, ae in rows:
+            t_n = next((lt for frags, lt in (loose or ()) if any(f in n for f in frags)), tol)
+            assert e < t_n, (n, e, t_n)
+    return rows[0][0]
 
 
-def _run_loss_and_grads(m, x0, x_t, cond, t, pt):
-    from diffsound_b200.modeling.transformers.diffusion_transformer import denoiser_loss
-    for p in m.parameters():
-        p.requires_grad_(True)
-        p.grad = None
-    names, params = zip(*m.transformer.named_parameters())
-    loss, prob, vb, hits = denoiser_loss(m, x0, x_t, cond, t, pt, True, True)
-    loss.backward()
-    return loss.detach(), prob, {n: p.grad for n, p in zip(names, params)}
+# (loss, gradient, log_model_prob): 4x the errors measured on an H100 80GB HBM3 (700 W) -- tf32 loss 2.3e-6, prob 1.4e-5, gradient 1.6e-3;
+# bf16 loss 8.0e-6, prob 9.7e-5, gradient 8.5e-2 -- where that is tighter than the parametrised bound (prob: 5e-3 tf32, 5e-2 bf16)
+TINY_MEASURED_TOL = {"tf32": (9.2e-6, 6.5e-3, 5.6e-5), "bf16": (3.2e-5, 3.4e-1, 3.9e-4)}
 
 
 @pytest.mark.parametrize("precision,tol_loss,tol_grad", [("tf32", 2e-3, 2e-2), ("bf16", 2e-2, 1.2e-1)])
 def test_tiny_training_step_matches_reference_loss_and_gradients(G, TO, precision, tol_loss, tol_grad):
     """Reference golden (unmodified DiffusionTransformer.forward(return_loss=True) + autograd, 2 layers, D=128)."""
+    m_loss, m_grad, m_prob = TINY_MEASURED_TOL[precision]
+    tol_prob = min(5e-3 if precision == "tf32" else 5e-2, m_prob)
+    lt_rtol = 10 * tol_loss
+    tol_loss, tol_grad = min(tol_loss, m_loss), min(tol_grad, m_grad)
     sd, gx = load_golden("xf_tiny.npz")
     _, g = load_golden("train_tiny.npz")
     K, D, NL, NH, CD, B, L = [int(v) for v in gx["__cfg"]]
@@ -238,29 +241,55 @@ def test_tiny_training_step_matches_reference_loss_and_gradients(G, TO, precisio
     x0 = torch.from_numpy(g["in_x0"]).long().cuda()
     t, pt = torch.from_numpy(g["in_t"]).cuda(), torch.from_numpy(g["in_pt"]).cuda()
     x_t = TO.q_sample(x0, t, torch.from_numpy(g["in_uniform"]).cuda(), m._sched(), 100)
-    loss, prob, grads = _run_loss_and_grads(m, x0, x_t, torch.from_numpy(g["in_cond"]).cuda(), t, pt)
+    loss, prob, grads = G.run_loss_and_grads(m, x0, x_t, torch.from_numpy(g["in_cond"]).cuda(), t, pt)
     ref_loss = float(g["out_loss"])
-    print(f"[{precision}] loss {float(loss):.6f} vs reference {ref_loss:.6f}")
-    assert abs(float(loss) - ref_loss) <= tol_loss * abs(ref_loss)
-    assert float((prob.cpu() - torch.from_numpy(g["out_probs"])).abs().max()) < (5e-3 if precision == "tf32" else 5e-2)
-    _grad_report(precision, grads, lambda n: torch.from_numpy(g["grad.transformer." + n]), tol_grad)
-    assert torch.allclose(m.Lt_history.cpu(), torch.from_numpy(g["out_Lt_history"]), rtol=10 * tol_loss, atol=1e-3)
+    e_loss = abs(float(loss) - ref_loss) / abs(ref_loss)
+    e_prob = float((prob.cpu() - torch.from_numpy(g["out_probs"])).abs().max())
+    e_grad = _grad_report(precision, grads, lambda n: torch.from_numpy(g["grad.transformer." + n]), None)
+    print(f"MEASURED tiny-{precision}: loss {float(loss):.6f} vs reference {ref_loss:.6f}, rel {e_loss:.3e}; prob {e_prob:.3e}; worst gradient rel {e_grad:.3e}")
+    assert e_loss <= tol_loss and e_prob <= tol_prob and e_grad <= tol_grad
+    assert torch.allclose(m.Lt_history.cpu(), torch.from_numpy(g["out_Lt_history"]), rtol=lt_rtol, atol=1e-3)
 
 
 def test_midsize_training_step_matches_oracle_autograd(G, TO):
-    """D=256 / 4 heads / 3 layers / K=64, B=4: every parameter gradient vs torch autograd through the oracle (CPU fp32)."""
-    K, D, NL, NH, CD, B, L = 64, 256, 3, 4, 96, 4, 265
+    """D=256 / 4 heads / 3 layers / K=64, B=4: every parameter gradient vs torch autograd through the oracle (CPU fp32).
+    Tolerances: 4x the errors measured on an H100 80GB HBM3 (700 W): loss 3.7e-6 (was 2e-3), gradient 3.1e-3 (was 2e-2)."""
+    _oracle_step(G, TO, "midsize", 64, 256, 3, 4, 96, torch.tensor([3, 0, 77, 99]), torch.tensor([0.01, 0.02, 0.005, 0.01]), "tf32", 1.5e-5, 1.25e-2)
+
+
+# bf16 full width, per parameter group, 4x the worst error measured in the group on an H100 80GB HBM3 (700 W).  The attention query and key
+# parameters get their gradients only through dS = scale P (dP - Delta), and with near-uniform scores at initialisation dP - Delta is a small
+# difference of bf16-rounded terms.  The key biases have exactly zero gradient (their error is over the 1e-4 floor): measured 0.45.  The query
+# weights / biases and key weights: 0.19.  Every other parameter: 8.1e-3, so an entirely wrong or zeroed gradient (error 1) fails.
+FULL_BF16_GROUPS = [((".key.bias",), 1.8), ((".query.", ".key.weight"), 0.77)]
+FULL_BF16_REST = 3.3e-2
+
+
+@pytest.mark.parametrize("precision,tol_loss,tol_grad", [("tf32", 6.2e-6, 5e-2), ("bf16", 3.4e-5, 1.8)])
+def test_full_width_training_step_matches_oracle_autograd(G, TO, precision, tol_loss, tol_grad):
+    """The width the benchmark trains: D=1024 / 16 heads / hidden 4096 / 2 layers / K=256, B=2, 77 condition tokens.
+    Tolerances: 4x the errors measured on an H100 80GB HBM3 (700 W): tf32 loss 1.5e-6, every gradient 1.2e-2; bf16 loss 8.5e-6, gradients
+    per parameter group (FULL_BF16_GROUPS; the parametrised 1.8 is the key-bias group's bound)."""
+    loose = None
+    if precision == "bf16":
+        assert FULL_BF16_GROUPS[0][1] == tol_grad
+        loose, tol_grad = FULL_BF16_GROUPS, FULL_BF16_REST
+    _oracle_step(G, TO, f"full-{precision}", 256, 1024, 2, 16, 512, torch.tensor([3, 77]), torch.tensor([0.01, 0.005]), precision, tol_loss, tol_grad,
+                 loose=loose)
+
+
+def _oracle_step(G, TO, tag, K, D, NL, NH, CD, t, pt, precision, tol_loss, tol_grad, loose=None):
+    B, L = t.numel(), 265
     sd = O.make_transformer_state_dict(K=K, D=D, n_layer=NL, n_head=NH, cond_dim=CD, seed=3)
     gen = torch.Generator().manual_seed(5)
     for k in sd:
         if k.endswith("bias") or "ln2.weight" in k or "to_logits.0.weight" in k:
             sd[k] = sd[k] + 0.05 * torch.randn(sd[k].shape, generator=gen)
     m = build_dt(K, D, NL, NH, CD, sd=sd)
-    m.transformer.train_engine.__init__(m.transformer, precision="tf32")
+    m.transformer.train_engine.__init__(m.transformer, precision=precision)
     cond = torch.randn(B, 77, CD, generator=gen)
     cond = cond / cond.norm(dim=-1, keepdim=True)
     x0 = torch.randint(0, K, (B, L), generator=gen)
-    t, pt = torch.tensor([3, 0, 77, 99]), torch.tensor([0.01, 0.02, 0.005, 0.01])
     u = portable_uniform(9, (B, K + 1, L))
     names = [n for n in sd if n.startswith("transformer.") and "attn2.mask" not in n]
     leaf = {k: (v.clone().requires_grad_(True) if k in names else v) for k, v in sd.items()}
@@ -269,11 +298,15 @@ def test_midsize_training_step_matches_oracle_autograd(G, TO):
     ref["loss"].backward()
     x_t = TO.q_sample(x0.cuda(), t.cuda(), u.cuda(), m._sched(), 100)
     assert torch.equal(x_t.cpu(), ref["x_t"])
-    loss, prob, grads = _run_loss_and_grads(m, x0.cuda(), x_t, cond.cuda(), t.cuda(), pt.cuda())
+    loss, prob, grads = G.run_loss_and_grads(m, x0.cuda(), x_t, cond.cuda(), t.cuda(), pt.cuda())
     rl = float(ref["loss"].detach())
-    print(f"midsize loss {float(loss):.6f} vs oracle {rl:.6f}")
-    assert abs(float(loss) - rl) <= 2e-3 * abs(rl)
-    _grad_report("midsize", grads, lambda n: leaf["transformer." + n].grad, 2e-2)
+    e_loss = abs(float(loss) - rl) / abs(rl)
+    e_grad = _grad_report(tag, grads, lambda n: leaf["transformer." + n].grad, None)
+    if loose is not None:  # per-parameter tolerances; the worst-error print above is the record
+        _grad_report(tag, grads, lambda n: leaf["transformer." + n].grad, tol_grad, loose=loose)
+        tol_grad = float("inf")
+    print(f"MEASURED {tag}: loss {float(loss):.6f} vs oracle {rl:.6f}, rel {e_loss:.3e}; worst gradient rel {e_grad:.3e}")
+    assert e_loss <= tol_loss and e_grad <= tol_grad
 
 
 def test_module_forward_backward_and_optimizer_steps(G, TO):

@@ -5,18 +5,13 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from oracle import diffsound_oracle as O  # noqa: E402
-from tests.helpers import load_golden, rel_err  # noqa: E402
+from tests.helpers import build_dt, load_golden, rel_err  # noqa: E402,F401  (build_dt: also imported from here by other test modules)
 
 
 @pytest.fixture(scope="module")
 def G():
     from tests import gpu_common
     return gpu_common
-
-
-def build_dt(K, D, NL, NH, CD, sd=None, spatial=(5, 53), T=100, precision="f16"):
-    from diffsound_b200.utils.builders import build_diffusion_transformer
-    return build_diffusion_transformer(K, D, NL, NH, CD, sd, spatial=spatial, T=T, precision=precision)
 
 
 def test_state_dict_keys_match_reference_golden(G):
