@@ -106,6 +106,9 @@ typedef struct dsb_gemm_desc {
                             with DSB_GEMM_NO_STORE) -- used once, at pack time, to calibrate the power-of-two activation scales of the fp16 MelGAN path */
   int resident_w;        /* 1: narrow-channel conv form (MelGAN's 64- and 32-channel stages, vocoder/modules.py:104-126): every tap is ONE 64-deep
                             k-block (K == 64), N <= 128.  2-byte dtypes, K-major operands, W not batched; runs on the same kernel as every other GEMM */
+  int schedule;          /* 0 = auto, 1 = data-parallel only.  Auto splits tiles between neighbouring CTAs (ordered stream-K) when the tiles leave a
+                            partial last wave; the output bits are the same either way.  Stream-K uses a per-device workspace, so at most one
+                            dsb_gemm_ex launch may be in flight per device at a time. */
 } dsb_gemm_desc;
 int dsb_gemm_ex(const dsb_gemm_desc* desc, void* stream);
 

@@ -26,6 +26,7 @@ class GemmDesc(C.Structure):
         ("use_tap_wcol", c_i), ("tap_wcol", c_i * 32), ("w_cols", c_ll), ("split_off", c_ll),
         ("dual_off", c_ll), ("out_col_group", c_i), ("out_col_group_stride", c_i), ("A2", c_vp),
         ("a2_rows", c_ll), ("a2_cols", c_ll), ("lda2", c_ll), ("a2_batch_stride", c_ll), ("tap_a2", c_i * 32), ("amax_out", c_vp), ("resident_w", c_i),
+        ("schedule", c_i),
     ]
 
 

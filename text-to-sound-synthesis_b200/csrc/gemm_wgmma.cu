@@ -12,12 +12,20 @@
 //   residual / tf32-round -> HBM) while the producer already streams the next tile's k-blocks into the smem ring.
 // * split-fp16 ("f16x3") form: one stage holds the four tiles of a k-block (A hi, A lo, W hi, W lo) and the consumers run the three passes
 //   lo*hi, hi*lo, hi*hi off that single staged copy.
+// * tile schedule (stream_k.cuh): data-parallel, or, when the tiles leave a partial last wave, ordered stream-K -- a tile may be split
+//   between two neighbouring CTAs at a k-block boundary.  The CTA holding the first k-blocks stores its fp32 accumulator to a per-device
+//   workspace; the CTA holding the rest loads it and continues the same accumulation sequence (the same FADDs / wgmma accumulations in the
+//   same order), then runs the epilogue.  Every output bit is what the data-parallel schedule computes.
+//   Contract: the workspace is shared by all launches on a device, so at most one GEMM may be in flight per device at a time (every caller
+//   issues its GEMMs on one stream; warm-up side streams are joined before and after).
 #include "common.cuh"
 #include "diffsound_b200.h"
+#include "stream_k.cuh"
 #include "wgmma.cuh"
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cstdlib>
+#include <mutex>
 #include <type_traits>
 
 namespace dsb {
@@ -62,7 +70,15 @@ struct GemmParams {
   // MN-major operands (2-byte types, one tap): the operand lies in HBM as (K rows, MN columns).  Loaded as 64-column x 64-row TMA boxes
   // (SWIZZLE_128B), consumed through MN-major (transposed) wgmma descriptors: no transposed copies.
   int a_mn, b_mn;
+  // ordered stream-K (stream_k.cuh): sk_part holds one BLOCK_N / 128 x 64 KB accumulator slot per CTA, sk_flag[c] = 1 once CTA c's slot is
+  // published (reset to 0 by its reader, so the workspace is clean again when the launch ends)
+  int stream_k;
+  float* sk_part;
+  int* sk_flag;
 };
+
+constexpr int SK_SLOT_FLOATS = 128 * 128;  // one 128 x 128 fp32 accumulator; a 256-wide tile uses two
+constexpr unsigned SK_SPIN_LIMIT = 1u << 24;  // ~ seconds of polling at 64 ns per try: far beyond any real wait, so only a protocol bug traps
 
 template <int BLOCK_N, bool F3>
 struct GemmSmem {
@@ -303,6 +319,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const int num_tiles = p.tiles_m * p.tiles_n * p.batch;
   // k-blocks per tile: (tap, channel block) pairs; the f16x3 form runs kb_per_tap blocks for each spatial tap
   const int num_kb = F3 ? p.kb_per_tap * p.f3_nsp : p.kb_per_tap * p.num_taps;
+  const dsb_sk::Work work = dsb_sk::cta_work(num_tiles, num_kb, gridDim.x, blockIdx.x, p.stream_k != 0);
+  const int n_pieces = dsb_sk::num_pieces(work);
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_a);
@@ -325,11 +343,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile % p.tiles_m;
-        const int n_blk = (tile / p.tiles_m) % p.tiles_n;
-        const int b = tile / (p.tiles_m * p.tiles_n);
-        for (int kb = 0; kb < num_kb; ++kb) {
+      for (int pi = 0; pi < n_pieces; ++pi) {
+        const dsb_sk::Piece pc = dsb_sk::piece(work, num_kb, pi);
+        const int m_blk = pc.tile % p.tiles_m;
+        const int n_blk = (pc.tile / p.tiles_m) % p.tiles_n;
+        const int b = pc.tile / (p.tiles_m * p.tiles_n);
+        for (int kb = pc.kb0; kb < pc.kb1; ++kb) {
           const int tap = kb / p.kb_per_tap;
           const int c0 = (kb - tap * p.kb_per_tap) * p.block_k;
           mbar_wait(&empty_bar[stage], phase ^ 1);
@@ -371,17 +390,38 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                         ((reinterpret_cast<uintptr_t>(p.out) & (4 * ((p.flags & (DSB_GEMM_OUT_F16_SPLIT | DSB_GEMM_OUT_F16 | DSB_GEMM_OUT_BF16)) ? 2 : 4) - 1)) == 0) &&
                         (!p.residual || (((p.ld_res & 3) == 0) && ((p.res_bstride & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0))) &&
                         (!p.bias || ((reinterpret_cast<uintptr_t>(p.bias) & 15) == 0));
+    const int ct = threadIdx.x - 128;  // consumer thread 0..255: its accumulator fragment's place in a stream-K slot
     int stage = 0;
     uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m_blk = tile % p.tiles_m;
-      const int n_blk = (tile / p.tiles_m) % p.tiles_n;
-      const int b = tile / (p.tiles_m * p.tiles_n);
+    for (int pi = 0; pi < n_pieces; ++pi) {
+      const dsb_sk::Piece pc = dsb_sk::piece(work, num_kb, pi);
+      const int m_blk = pc.tile % p.tiles_m;
+      const int n_blk = (pc.tile / p.tiles_m) % p.tiles_n;
+      const int b = pc.tile / (p.tiles_m * p.tiles_n);
       float acc[NH][64];
+      const bool tail = pc.kb0 > 0;  // stream-K tail: continue from the accumulator CTA blockIdx.x - 1 published for k-blocks [0, kb0)
+      if (tail) {
+        if (ct == 0) {
+          int* flag = p.sk_flag + blockIdx.x - 1;
+          unsigned spins = 0;
+          while (ld_acquire_gpu(flag) == 0) {
+            if (++spins > SK_SPIN_LIMIT) __trap();
+            __nanosleep(64);
+          }
+          *flag = 0;  // consumed: the next launch finds the flag clear
+        }
+        named_bar_sync(1, 256);
+      }
+      {
+        const float4* slot = reinterpret_cast<const float4*>(p.sk_part + (size_t)(blockIdx.x - 1) * NH * SK_SLOT_FLOATS);
 #pragma unroll
-      for (int h = 0; h < NH; ++h)
+        for (int h = 0; h < NH; ++h)
 #pragma unroll
-        for (int i = 0; i < 64; ++i) acc[h][i] = 0.f;
+          for (int q = 0; q < 16; ++q) {
+            const float4 v = tail ? __ldcg(slot + (h * 16 + q) * 256 + ct) : make_float4(0.f, 0.f, 0.f, 0.f);  // __ldcg: L2, not a stale L1 line
+            acc[h][4 * q] = v.x; acc[h][4 * q + 1] = v.y; acc[h][4 * q + 2] = v.z; acc[h][4 * q + 3] = v.w;
+          }
+      }
       int prev_stage = -1;
       if constexpr (F3) {
         // parity-grade form: the wgmma accumulator does not round every addition like an fp32 FADD, which over K = 4096 costs more than
@@ -389,7 +429,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         // The pipe drains once per k-block for this.  Overlapping the promotion with the next k-block (two partial accumulators,
         // wgmma_wait<1>) measured slower on an H100, see DESIGN section 4.
         float part[64];
-        for (int kb = 0; kb < num_kb; ++kb) {
+        for (int kb = pc.kb0; kb < pc.kb1; ++kb) {
           mbar_wait(&full_bar[stage], phase);
           const uint32_t sa = smem_u32(smem + stage * S::STAGE_BYTES);
           wgmma_fence_regs(part);
@@ -407,8 +447,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       } else {
         // the MN-major choice is made once per tile, outside the wgmma window: a branch between wgmma_fence and commit makes
         // ptxas inject warpgroup.arrive (C7519) around every MMA
+        // kb is absolute, so a stream-K tail's first k-block accumulates onto the loaded partial (scale-d = 1)
         auto mainloop = [&](auto ta, auto tb) {
-          for (int kb = 0; kb < num_kb; ++kb) {
+          for (int kb = pc.kb0; kb < pc.kb1; ++kb) {
             mbar_wait(&full_bar[stage], phase);
             const uint32_t sa = smem_u32(smem + stage * S::STAGE_BYTES);
 #pragma unroll
@@ -437,6 +478,19 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 #pragma unroll
       for (int h = 0; h < NH; ++h) wgmma_fence_regs(acc[h]);
       if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+      if (pc.kb1 < num_kb) {
+        // stream-K head (this CTA's first piece): publish the partial accumulator to slot blockIdx.x for CTA blockIdx.x + 1
+        float4* slot = reinterpret_cast<float4*>(p.sk_part + (size_t)blockIdx.x * NH * SK_SLOT_FLOATS);
+#pragma unroll
+        for (int h = 0; h < NH; ++h)
+#pragma unroll
+          for (int q = 0; q < 16; ++q) __stcg(slot + (h * 16 + q) * 256 + ct, make_float4(acc[h][4 * q], acc[h][4 * q + 1], acc[h][4 * q + 2], acc[h][4 * q + 3]));
+        __threadfence();
+        named_bar_sync(1, 256);
+        if (ct == 0) st_release_gpu(p.sk_flag + blockIdx.x, 1);
+        continue;
+      }
 
       // ---- epilogue: accumulator fragment (rows lane/4 and lane/4 + 8 of this warp's 16, columns 8j + 2(lane%4) + {0,1}) -> smem chunk -> stores
       const int row_base = m_blk * BLOCK_M + wg * 64 + wq * 16;
@@ -520,8 +574,32 @@ int make_operand_map_mn(CUtensorMap* map, const void* ptr, int kind, long long m
   return 0;
 }
 
+// The stream-K workspace of the current device: one 256-wide accumulator slot per SM, then one flag per SM.  Allocated zeroed on the first
+// call that is not being captured into a CUDA graph; until then (a first call inside a capture) the caller runs data-parallel.
+static int sk_workspace(cudaStream_t st, float** part, int** flag) {
+  static std::mutex mu;
+  static void* ws[64] = {};
+  int dev = 0;
+  DSB_CHECK_CUDA(cudaGetDevice(&dev));
+  DSB_REQUIRE(dev < 64, "dsb_gemm_ex: device %d out of range for the stream-K workspace", dev);
+  std::lock_guard<std::mutex> lock(mu);
+  if (!ws[dev]) {
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    DSB_CHECK_CUDA(cudaStreamIsCapturing(st, &cap));
+    if (cap != cudaStreamCaptureStatusNone) return 0;
+    const size_t bytes = (size_t)sm_count() * (2 * SK_SLOT_FLOATS * sizeof(float) + sizeof(int));
+    void* w = nullptr;
+    DSB_CHECK_CUDA(cudaMalloc(&w, bytes));
+    DSB_CHECK_CUDA(cudaMemsetAsync(w, 0, bytes, st));
+    ws[dev] = w;
+  }
+  *part = static_cast<float*>(ws[dev]);
+  *flag = reinterpret_cast<int*>(*part + (size_t)sm_count() * 2 * SK_SLOT_FLOATS);
+  return 0;
+}
+
 template <int BLOCK_N, int KIND, bool F3>
-static int launch(const CUtensorMap& ma, const CUtensorMap& ma2, const CUtensorMap& mb, const GemmParams& p, int max_ctas, cudaStream_t st) {
+static int launch(const CUtensorMap& ma, const CUtensorMap& ma2, const CUtensorMap& mb, GemmParams& p, int max_ctas, int schedule, cudaStream_t st) {
   using S = GemmSmem<BLOCK_N, F3>;
   auto kern = gemm_wgmma_kernel<BLOCK_N, KIND, F3>;
   static bool attr_done = false;
@@ -531,6 +609,12 @@ static int launch(const CUtensorMap& ma, const CUtensorMap& ma2, const CUtensorM
   }
   const int tiles = p.tiles_m * p.tiles_n * p.batch;
   int grid = tiles < max_ctas ? tiles : max_ctas;
+  const int num_kb = F3 ? p.kb_per_tap * p.f3_nsp : p.kb_per_tap * p.num_taps;
+  p.stream_k = 0;
+  if (schedule == 0 && dsb_sk::stream_k_applies(tiles, num_kb, grid, sm_count())) {
+    if (int r = sk_workspace(st, &p.sk_part, &p.sk_flag)) return r;
+    p.stream_k = p.sk_part != nullptr;
+  }
   DSB_CHECK_CUDA(launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), S::TOTAL, st, ma, ma2, mb, p));
   return 0;
 }
@@ -593,6 +677,7 @@ extern "C" int dsb_gemm_ex(const dsb_gemm_desc* d, void* stream) {
     DSB_REQUIRE(kind != DSB_DTYPE_TF32 && !any_mn && !p.b_batched && d->K == 64 && d->N <= 128 && d->use_tap_wcol,
                 "dsb_gemm_ex: resident_w needs a 2-byte dtype, K-major operands, K == 64 per tap, N <= 128, explicit tap_wcol and an unbatched W");
   DSB_REQUIRE(!(any_mn && d->cta_pair > 0), "dsb_gemm_ex: 256 x 256 pair tiles take K-major operands only");
+  DSB_REQUIRE(d->schedule == 0 || d->schedule == 1, "dsb_gemm_ex: schedule must be 0 (auto) or 1 (data-parallel only)");
 
   const int sms = sm_count();
   const int max_ctas = d->max_ctas > 0 ? d->max_ctas : sms;
@@ -648,14 +733,14 @@ extern "C" int dsb_gemm_ex(const dsb_gemm_desc* d, void* stream) {
       const int sh = p.tap_shift[3 * j], ac = p.tap_acol[3 * j + 1], wc = p.tap_wcol[3 * j];
       p.tap_shift[j] = sh; p.tap_acol[j] = ac; p.tap_wcol[j] = wc;
     }
-    return launch<128, DSB_DTYPE_F16, true>(ma, ma2, mb, p, max_ctas, st);
+    return launch<128, DSB_DTYPE_F16, true>(ma, ma2, mb, p, max_ctas, d->schedule, st);
   }
   if (block_n == 256) {
-    if (kind == DSB_DTYPE_TF32) return launch<256, DSB_DTYPE_TF32, false>(ma, ma2, mb, p, max_ctas, st);
-    if (kind == DSB_DTYPE_BF16) return launch<256, DSB_DTYPE_BF16, false>(ma, ma2, mb, p, max_ctas, st);
-    return launch<256, DSB_DTYPE_F16, false>(ma, ma2, mb, p, max_ctas, st);
+    if (kind == DSB_DTYPE_TF32) return launch<256, DSB_DTYPE_TF32, false>(ma, ma2, mb, p, max_ctas, d->schedule, st);
+    if (kind == DSB_DTYPE_BF16) return launch<256, DSB_DTYPE_BF16, false>(ma, ma2, mb, p, max_ctas, d->schedule, st);
+    return launch<256, DSB_DTYPE_F16, false>(ma, ma2, mb, p, max_ctas, d->schedule, st);
   }
-  if (kind == DSB_DTYPE_TF32) return launch<128, DSB_DTYPE_TF32, false>(ma, ma2, mb, p, max_ctas, st);
-  if (kind == DSB_DTYPE_BF16) return launch<128, DSB_DTYPE_BF16, false>(ma, ma2, mb, p, max_ctas, st);
-  return launch<128, DSB_DTYPE_F16, false>(ma, ma2, mb, p, max_ctas, st);
+  if (kind == DSB_DTYPE_TF32) return launch<128, DSB_DTYPE_TF32, false>(ma, ma2, mb, p, max_ctas, d->schedule, st);
+  if (kind == DSB_DTYPE_BF16) return launch<128, DSB_DTYPE_BF16, false>(ma, ma2, mb, p, max_ctas, d->schedule, st);
+  return launch<128, DSB_DTYPE_F16, false>(ma, ma2, mb, p, max_ctas, d->schedule, st);
 }

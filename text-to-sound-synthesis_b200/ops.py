@@ -145,10 +145,11 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
          lrelu: bool = False, tanh: bool = False, res_before_act: bool = False, taps: Optional[Sequence[int]] = None,
          tap_acol: Optional[Sequence[int]] = None, k_per_tap: Optional[int] = None, out_rows: Optional[int] = None, geo: Optional[Sequence[int]] = None, alpha: float = 1.0,
          block_n: int = 0, max_ctas: int = 0, cta_pair: int = 0, a_mn: bool = False, w_mn: bool = False,
-         tap_wcol: Optional[Sequence[int]] = None, split_out: bool = False) -> torch.Tensor:
+         tap_wcol: Optional[Sequence[int]] = None, split_out: bool = False, schedule: int = 0) -> torch.Tensor:
     """out = epi(alpha * A @ W^T + bias) (+ residual) on the tensor cores (wgmma).  a: (M,K) or (batch,M,K); w: (N, taps*K) or (batch,N,K).
     a_mn / w_mn: that operand is given MN-major, i.e. as it lies in memory with the reduction dimension as rows -- a: (K, M), w: (K, N)
-    (2-byte dtypes): out = a^T @ w with no transposed copies."""
+    (2-byte dtypes): out = a^T @ w with no transposed copies.
+    schedule: 0 = auto (ordered stream-K when the tiles leave a partial last wave), 1 = data-parallel only; the output bits are the same."""
     _need_cuda(a, w, bias, residual, out)
     batched = a.dim() == 3
     if a.stride(-1) != 1 or w.stride(-1) != 1:
@@ -197,13 +198,15 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
     d.alpha = alpha
     d.block_n, d.max_ctas, d.cta_pair = block_n, max_ctas, cta_pair
     d.a_mn_major, d.b_mn_major = int(a_mn), int(w_mn)
+    d.schedule = schedule
     _lib.check(_lib.lib().dsb_gemm_ex(C.byref(d), _stream()), "dsb_gemm_ex")
     return out
 
 
 def gemm_desc(*, A, W, out, M, N, K, taps, lda, ldw, ldo, dtype=F16, batch=1, a_rows=0, a_cols=0, a_batch_stride=0, w_cols=0, out_batch_stride=0,
               bias=None, flags=0, alpha=1.0, split_off=0, dual_off=0, out_col_group=0, out_col_group_stride=0, A2=None, lda2=0, a2_rows=0, a2_cols=0,
-              a2_batch_stride=0, block_n=0, cta_pair=0, residual=None, ld_res=0, geo=None, amax_out=None, resident_w=0):
+              a2_batch_stride=0, block_n=0, cta_pair=0, residual=None, ld_res=0, geo=None, amax_out=None, resident_w=0,
+              schedule=0):
     """Thin front end of dsb_gemm_ex for callers that lay out their own buffers (the MelGAN / SpecVQGAN state buffers): A / W / out / A2 are
     raw device addresses (ints: tensor.data_ptr() plus a byte offset), sizes and strides in elements; taps = [(row_shift, a_col, w_col, use_a2), ...]."""
     d = _lib.GemmDesc()
@@ -222,6 +225,7 @@ def gemm_desc(*, A, W, out, M, N, K, taps, lda, ldw, ldo, dtype=F16, batch=1, a_
     d.residual, d.ld_res = residual, ld_res
     d.amax_out = _ptr(amax_out)
     d.resident_w = int(resident_w)
+    d.schedule = schedule
     if geo is not None:
         d.geo_P, d.geo_Wp, d.geo_y0, d.geo_y1, d.geo_x0, d.geo_x1 = [int(v) for v in geo]
     _lib.check(_lib.lib().dsb_gemm_ex(C.byref(d), _stream()), "dsb_gemm_ex")
