@@ -41,6 +41,7 @@ extern "C" {
 #define DSB_GEMM_DUAL_LRELU 4096 /* with OUT_F16_SPLIT: also store the pair of LeakyReLU(0.2)(x) at +dual_off (reference vocoder/modules.py:76: the
                                    next ResnetBlock convolves the activated signal while its 1x1 shortcut reads the raw one) */
 #define DSB_GEMM_NO_STORE 16384 /* run the GEMM and its epilogue but store nothing (amax_out calibration pass) */
+#define DSB_GEMM_RELU 32768   /* max(x, 0), NaN passes through     (torchvision inception.py BasicConv2d, Melception's every conv) */
 #define DSB_GEMM_OUT_F16_SPLIT 2048 /* store the fp16 (hi | lo) pair of the fp32 result: hi = f16(x) at out[r*ldo + c], lo = f16(x - hi) at
                                        out[r*ldo + split_off + c] -- the A operand of a split-fp16 ("f16x3") GEMM, see dsb_split_f16 */
 /* GroupNorm-apply flags (share the ROUND_TF32 bit) */
@@ -280,6 +281,37 @@ int dsb_edge_pad_f16(void* state_f16, long long ld, long long batch_stride, int 
 int dsb_conv_out_pair(const void* state, long long ld, long long batch_stride, int B, int T, int row0, int col0, int cs, int kt, const float* w,
                       const float* bias, float scale, float* out, void* stream);
 
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * Melception feature extractor support (reference Codebook/evaluation/feature_extractors/melception.py:23-113 over torchvision's Inception3).
+ * Activations are split-fp16 PAIR IMAGES: channels-last fp16 (B, Hp, Wp, ld) whose pixel rows hold hi = f16(v) at [0, C) and lo = f16(v - hi)
+ * at [lo_off, lo_off + C), on a zero-bordered grid; a tensor's valid pixels are a window [y0, y0 + H) x [x0, x0 + W) of that grid and every
+ * other pixel is zero.  Where an argument list has no ld / lo_off for a tensor, its rows are [hi C | lo C].  Every convolution except the stem
+ * is a dsb_gemm_ex over such images (row-shift taps, the geo_* window mask, DSB_GEMM_RELU, DSB_GEMM_OUT_F16_SPLIT into a channel slice).
+ * ------------------------------------------------------------------------------------------------------------- */
+/* Conv2d_1a_3x3 (1 -> Cout, 3x3, stride 2, valid) with its BatchNorm folded into w (Cout, 9) / bias (Cout), ReLU, times the power of two `scale`:
+ * x (B, F, T) fp32 mels, optionally normalised per mel bin first, (x - mean[f]) / stdv[f] (mean = stdv = NULL: none).  Writes the whole
+ * (B, Hp, Wp, 2 Cout) pair grid: the ((F-3)/2+1) x ((T-3)/2+1) output window at (y0, x0), zeros elsewhere. */
+int dsb_mel_stem(const float* x, const float* mean, const float* stdv, const float* w, const float* bias, float scale, void* out, int B, int F, int T,
+                 int Cout, int Hp, int Wp, int y0, int x0, void* stream);
+/* Stride-2 phases of a pair image (the fp16-pair form of dsb_space_to_depth_padded, for 3x3 stride-2 VALID convs): in (B, Hpi, Wpi, 2C), window
+ * (y0, x0, H, W) -> out (B, Hpo, Wpo, 8C), rows [hi of phases 0..3 | lo of phases 0..3], phase ph = 2 py + px of pixel (oy0 + u, ox0 + v) holding
+ * window pixel (2u + py, 2v + px) (zero outside the window).  The conv is then a 9-tap GEMM with row shifts (dy/2) Wpo + dx/2 and A column
+ * offsets (2 (dy%2) + dx%2) C.  A pure copy: bit-exact.  C % 8 == 0. */
+int dsb_pair_space_to_depth(const void* in, int Hpi, int Wpi, int y0, int x0, int H, int W, void* out, int Hpo, int Wpo, int oy0, int ox0, int B, int C,
+                            void* stream);
+/* MaxPool2d(3, stride 2) of the window (y0, x0, H, W) of in (B, Hpi, Wpi, 2C) into the output window at (oy0, ox0) of the grid (B, Hpo, Wpo, ldo)
+ * (hi at column c, lo at lo_off + c; out may point into a channel slice of a concat), zeros elsewhere in that slice.  The winning pixel's pair is
+ * copied (times the power of two `scale`, which moves it to the concat's activation scale): exact. */
+int dsb_pair_maxpool3s2(const void* in, int Hpi, int Wpi, int y0, int x0, int H, int W, void* out, long long ldo, long long lo_off, int Hpo, int Wpo,
+                        int oy0, int ox0, int B, int C, float scale, void* stream);
+/* AvgPool2d(3, stride 1, padding 1, count_include_pad) over the window of in (B, Hp, Wp, 2C): sum of the nine (hi + lo) in fp32, / 9, re-split,
+ * into out (same grid, row stride ldo, lo at lo_off); zeros outside the window.  C % 4 == 0. */
+int dsb_pair_avgpool3(const void* in, int Hp, int Wp, int y0, int x0, int H, int W, void* out, long long ldo, long long lo_off, int B, int C, void* stream);
+/* adaptive_avg_pool2d(., 1) of a pair image: out (B, C) fp32 = inv_scale * mean over the window of (hi + lo), fp64 partial sums in a fixed order
+ * (deterministic).  inv_scale undoes the tensor's power-of-two activation scale exactly. */
+int dsb_pair_channel_mean(const void* in, long long ld, long long lo_off, int Hp, int Wp, int y0, int x0, int H, int W, int B, int C, float inv_scale,
+                          float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Training (SURVEY.md section 8 row A13; reference sound_synthesis/modeling/transformers/diffusion_transformer.py:370-377, :408-476).

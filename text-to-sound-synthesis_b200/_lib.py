@@ -66,6 +66,12 @@ SIGNATURES = {
     "dsb_posterior_sample": [c_vp] * 8 + [c_i] * 5 + [c_f, c_i, c_i, c_vp],
     "dsb_posterior_sample_loop": [c_vp] * 8 + [c_i] * 5 + [c_f, c_i, c_vp],
     "dsb_aten_uniform": [c_vp, c_ll, C.c_ulonglong, C.c_ulonglong, C.c_ulonglong, c_vp],
+    # Melception feature extractor
+    "dsb_mel_stem": [c_vp] * 5 + [c_f, c_vp] + [c_i] * 8 + [c_vp],
+    "dsb_pair_space_to_depth": [c_vp] + [c_i] * 6 + [c_vp] + [c_i] * 6 + [c_vp],
+    "dsb_pair_maxpool3s2": [c_vp] + [c_i] * 6 + [c_vp, c_ll, c_ll] + [c_i] * 6 + [c_f, c_vp],
+    "dsb_pair_avgpool3": [c_vp] + [c_i] * 6 + [c_vp, c_ll, c_ll, c_i, c_i, c_vp],
+    "dsb_pair_channel_mean": [c_vp, c_ll, c_ll] + [c_i] * 8 + [c_f, c_vp, c_vp],
     # training (A13)
     "dsb_q_sample": [c_vp] * 5 + [c_i] * 4 + [c_vp],
     "dsb_train_loss": [c_vp] * 16 + [c_i] * 4 + [c_f, c_i, c_f, c_f, c_i, c_vp],

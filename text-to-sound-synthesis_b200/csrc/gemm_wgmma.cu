@@ -96,7 +96,7 @@ struct GemmSmem {
 __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const float* sw, int row_base, int col0, int b, int lane, bool vec_ok) {
   const bool has_geo = p.geo_P > 0;
   const int out_mode = (p.flags & DSB_GEMM_OUT_F16_SPLIT) ? 3 : ((p.flags & DSB_GEMM_OUT_F16) ? 1 : ((p.flags & DSB_GEMM_OUT_BF16) ? 2 : 0));
-  const int act = (p.flags & DSB_GEMM_GELU2) ? 1 : ((p.flags & DSB_GEMM_LRELU) ? 2 : ((p.flags & DSB_GEMM_TANH) ? 3 : 0));
+  const int act = (p.flags & DSB_GEMM_GELU2) ? 1 : ((p.flags & DSB_GEMM_LRELU) ? 2 : ((p.flags & DSB_GEMM_TANH) ? 3 : ((p.flags & DSB_GEMM_RELU) ? 4 : 0)));
   const bool do_round = (p.flags & DSB_GEMM_ROUND_TF32) != 0;
   const bool dual = (p.flags & DSB_GEMM_DUAL_LRELU) != 0;
   const bool res_first = (p.flags & DSB_GEMM_RES_BEFORE_ACT) != 0;
@@ -149,6 +149,9 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const float*
         const float z = fminf(fmaxf(x[e], -15.f), 15.f);
         x[e] = 1.0f - __fdividef(2.0f, 1.0f + __expf(2.0f * z));
       }
+    } else if (act == 4) {
+#pragma unroll
+      for (int e = 0; e < 4 * NI; ++e) x[e] = x[e] < 0.f ? 0.f : x[e];  // a NaN passes through, as in torch.relu
     }
     if (res_b && !res_first) {
 #pragma unroll
@@ -244,6 +247,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const float*
         if (act == 1) xv = __fdividef(xv, 1.0f + __expf(-1.702f * xv));
         else if (act == 2) xv = xv > 0.f ? xv : 0.2f * xv;
         else if (act == 3) { const float z = fminf(fmaxf(xv, -15.f), 15.f); xv = 1.0f - __fdividef(2.0f, 1.0f + __expf(2.0f * z)); }
+        else if (act == 4) xv = xv < 0.f ? 0.f : xv;
         if (!res_first) xv += rv;
         if (do_round) xv = round_tf32(xv);
         if (!((in_mask >> i) & 1u)) xv = 0.f;

@@ -17,6 +17,7 @@ OUT_F16_SPLIT = 2048
 DUAL_LRELU = 4096
 SPLIT_OUT_F16 = 8192
 NO_STORE = 16384
+RELU = 32768
 
 
 def _stream() -> int:
@@ -142,7 +143,7 @@ def silu(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
 
 def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
          out: Optional[torch.Tensor] = None, *, dtype: int = TF32, gelu: bool = False, round_out: bool = False, out_bf16: bool = False, out_f16: bool = False,
-         lrelu: bool = False, tanh: bool = False, res_before_act: bool = False, taps: Optional[Sequence[int]] = None,
+         lrelu: bool = False, tanh: bool = False, relu: bool = False, res_before_act: bool = False, taps: Optional[Sequence[int]] = None,
          tap_acol: Optional[Sequence[int]] = None, k_per_tap: Optional[int] = None, out_rows: Optional[int] = None, geo: Optional[Sequence[int]] = None, alpha: float = 1.0,
          block_n: int = 0, max_ctas: int = 0, cta_pair: int = 0, a_mn: bool = False, w_mn: bool = False,
          tap_wcol: Optional[Sequence[int]] = None, split_out: bool = False, schedule: int = 0) -> torch.Tensor:
@@ -180,7 +181,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
     d.out_batch_stride = out.stride(0) if batched else 0
     d.res_batch_stride = residual.stride(0) if (residual is not None and batched) else 0
     d.dtype = dtype
-    d.flags = (GELU2 if gelu else 0) | (ROUND_TF32 if round_out else 0) | (OUT_BF16 if out_bf16 else 0) | (LRELU if lrelu else 0) | (TANH if tanh else 0) | (RES_BEFORE_ACT if res_before_act else 0) | (OUT_F16 if out_f16 else 0) | (OUT_F16_SPLIT if split_out else 0)
+    d.flags = (GELU2 if gelu else 0) | (ROUND_TF32 if round_out else 0) | (OUT_BF16 if out_bf16 else 0) | (LRELU if lrelu else 0) | (TANH if tanh else 0) | (RELU if relu else 0) | (RES_BEFORE_ACT if res_before_act else 0) | (OUT_F16 if out_f16 else 0) | (OUT_F16_SPLIT if split_out else 0)
     if split_out:
         d.split_off = N
     if tap_wcol is not None:
@@ -522,4 +523,55 @@ def lrelu_pad(x, pad, *, slope=0.2, reflect=True, channel_major=False, round_out
     out = torch.empty(B, T + 2 * pad, Co, dtype=torch.float32, device=x.device)
     _lib.check(_lib.lib().dsb_lrelu_pad(x.data_ptr(), out.data_ptr(), B, T, Cc, pad, slope, 1 if reflect else 0, 1 if channel_major else 0,
                                         SPLIT_OUT if split else (ROUND_TF32 if round_out else 0), _stream()), "dsb_lrelu_pad")
+    return out
+
+
+# ---------------------------------------------------------------------------------------------- Melception support (pair images, see the header)
+def mel_stem(x, w, bias, out, *, Hp, Wp, y0, x0, scale=1.0, mean=None, std=None):
+    """x (B, F, T) fp32 mels -> out (B, Hp, Wp, 2 Cout) fp16 pair grid of scale * relu(conv3x3_s2((x - mean) / std) + bias), zeros outside the window."""
+    _need_cuda(x, w, bias, out, mean, std)
+    x = x.contiguous()
+    B, F_, T = x.shape
+    _lib.check(_lib.lib().dsb_mel_stem(x.data_ptr(), _ptr(mean), _ptr(std), w.data_ptr(), bias.data_ptr(), float(scale), out.data_ptr(), B, F_, T, w.shape[0],
+                                       Hp, Wp, y0, x0, _stream()), "dsb_mel_stem")
+    return out
+
+
+def pair_space_to_depth(x, window, out, out_origin):
+    """x (B, Hpi, Wpi, 2C) pair image with window (y0, x0, H, W) -> its stride-2 phases in out (B, Hpo, Wpo, 8C) at out_origin (oy0, ox0)."""
+    _need_cuda(x, out)
+    B, Hpi, Wpi, C2 = x.shape
+    _lib.check(_lib.lib().dsb_pair_space_to_depth(x.data_ptr(), Hpi, Wpi, *window, out.data_ptr(), out.shape[1], out.shape[2], *out_origin, B, C2 // 2,
+                                                  _stream()), "dsb_pair_space_to_depth")
+    return out
+
+
+def pair_maxpool3s2(x, window, out, out_origin, *, out_ptr=None, ldo=None, lo_off=None, scale=1.0):
+    """MaxPool2d(3, 2) of x's window into out (B, Hpo, Wpo, ldo) at out_origin; out_ptr / lo_off address a channel slice of out (defaults: all of it)."""
+    _need_cuda(x, out)
+    B, Hpi, Wpi, C2 = x.shape
+    C = C2 // 2
+    _lib.check(_lib.lib().dsb_pair_maxpool3s2(x.data_ptr(), Hpi, Wpi, *window, out.data_ptr() if out_ptr is None else out_ptr, out.shape[-1] if ldo is None else ldo,
+                                              C if lo_off is None else lo_off, out.shape[1], out.shape[2], *out_origin, B, C, float(scale), _stream()),
+               "dsb_pair_maxpool3s2")
+    return out
+
+
+def pair_avgpool3(x, window, out=None):
+    """AvgPool2d(3, 1, 1) (count_include_pad) of x's window (B, Hp, Wp, 2C) -> out (same shape) pair image."""
+    _need_cuda(x, out)
+    B, Hp, Wp, C2 = x.shape
+    out = torch.empty_like(x) if out is None else out
+    _lib.check(_lib.lib().dsb_pair_avgpool3(x.data_ptr(), Hp, Wp, *window, out.data_ptr(), out.shape[-1], C2 // 2, B, C2 // 2, _stream()), "dsb_pair_avgpool3")
+    return out
+
+
+def pair_channel_mean(x, window, *, inv_scale=1.0, out=None):
+    """x (B, Hp, Wp, 2C) pair image -> (B, C) fp32 mean over the window, times inv_scale."""
+    _need_cuda(x, out)
+    B, Hp, Wp, C2 = x.shape
+    C = C2 // 2
+    out = torch.empty(B, C, dtype=torch.float32, device=x.device) if out is None else out
+    _lib.check(_lib.lib().dsb_pair_channel_mean(x.data_ptr(), C2, C, Hp, Wp, *window, B, C, float(inv_scale), out.data_ptr(), _stream()),
+               "dsb_pair_channel_mean")
     return out
