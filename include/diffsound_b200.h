@@ -179,8 +179,8 @@ int dsb_attention_tc(const void* q, long long ldq, const void* k, long long ldk,
 int dsb_attention_tc2(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* o, long long ldo,
                       int B, int H, int Lq, int Lk, float scale, void* stream);
 /* split-fp16 ("f16x3") version of the same core for the parity-grade mode: q / k / v / o are fp16 (hi | lo) pairs -- the lo half of a row
- * lies *_lo_off elements after its hi half -- S = Qhi Khi^T + Qlo Khi^T + Qhi Klo^T and O = Phi Vhi + Plo Vhi + Phi Vlo with mma.sync and fp32
- * accumulation; P = exp2(...) is split into (hi | lo) in registers.  Lk <= 288. */
+ * lies *_lo_off elements after its hi half -- S = Qhi Khi^T + Qlo Khi^T + Qhi Klo^T and O = Phi Vhi + Plo Vhi + Phi Vlo with wgmma and fp32
+ * accumulation; P = exp2(...) is split into (hi | lo) in registers.  q / k / v / o 16-byte aligned (TMA), any Lk. */
 int dsb_attention_tc_split(const void* q, long long ldq, long long q_lo_off, const void* k, long long ldk, long long k_lo_off, const void* v,
                            long long ldv, long long v_lo_off, void* o, long long ldo, long long o_lo_off, int B, int H, int Lq, int Lk,
                            float scale, void* stream);
