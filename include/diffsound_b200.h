@@ -223,6 +223,20 @@ int dsb_posterior_sample(const float* logits, const int64_t* x_t, const int64_t*
 int dsb_posterior_sample_loop(const float* logits, int64_t* x, int64_t* t, int64_t* t_post, const float* sched, unsigned long long* ctrl,
                               const int64_t* t_sched, const int64_t* t_post_sched, int B, int K, int L, int T, int trunc_mode, float trunc_r,
                               int trunc_k, void* stream);
+/* Wide forms of the two entry points above, for codebooks up to K = 4095 (the 2048-code AudioSet codebook has K + 1 = 2049 classes), with
+ * identical argument lists and the same contract: diffusion_transformer.py:285-289 (predict_start tail), dalle_spec.py:146-174 (top-k /
+ * nucleus truncation), diffusion_transformer.py:293-339 (q_posterior), :359-368 (log_sample_categorical); same stage flags, layouts,
+ * truncation key and predicate, first-index ties, t_post and clamp of t, log_prob_out, in-kernel replay of torch.rand_like and loop-control
+ * block.  One CTA of 256 threads per (b, l) column instead of one warp; the fp64 / fp32 reductions run in a fixed order that depends on
+ * nothing but the column (each thread in ascending k, a warp xor butterfly 16 ... 1, then the 8 warp partials in ascending warp order), so
+ * log-probs can differ from the warp kernel's in the last bit of a near-midpoint value and ids only at near ties.  Every K in [1, 4095] is
+ * accepted; K > 4095 is refused ("too large") before anything is launched.  B <= 65535. */
+int dsb_posterior_sample_wide(const float* logits, const int64_t* x_t, const int64_t* t, const int64_t* t_post, const float* uniform,
+                              const float* sched, int64_t* x_next, float* log_prob_out, int B, int K, int L, int T, int trunc_mode,
+                              float trunc_r, int trunc_k, int stage_flags, void* stream);
+int dsb_posterior_sample_wide_loop(const float* logits, int64_t* x, int64_t* t, int64_t* t_post, const float* sched, unsigned long long* ctrl,
+                                   const int64_t* t_sched, const int64_t* t_post_sched, int B, int K, int L, int T, int trunc_mode, float trunc_r,
+                                   int trunc_k, void* stream);
 /* out[i] = the i-th element torch.rand(n, device='cuda') would hold for generator state (seed, philox offset) with ATen's launch geometry
  * nthreads = 256 * min(SMs * (maxThreadsPerSM / 256), ceil(n / 256)); used by the tests to pin the replay against torch.rand itself. */
 int dsb_aten_uniform(float* out, long long n, unsigned long long seed, unsigned long long offset, unsigned long long nthreads, void* stream);
@@ -327,7 +341,8 @@ int dsb_q_sample(const int64_t* x0, const int64_t* t, const float* uniform, cons
  * Outputs: log_model_prob (B, K+1, L) or NULL (exp() of it when prob_as_exp: forward()'s out['logits'], :573-574); col_loss (B, L, 2) per-column (main, aux) terms; hits (B, L, 2) int flags
  *   (argmax(log_x0_recon) == x0, argmax(log_model_prob) == x_t; :424-433) or NULL; kl_loss (B), vb_loss (B), loss (1).
  * lt_history / lt_count (T floats each, updated in place as :448-454 does) may be NULL; scratch_b is B floats.
- * aux_weight = 0 disables the auxiliary term (is_train=False or auxiliary_loss_weight=0). */
+ * aux_weight = 0 disables the auxiliary term (is_train=False or auxiliary_loss_weight=0).
+ * K <= 4095: one warp per column up to K = 1055, one CTA of 256 threads per column above (block reductions in a fixed order). */
 int dsb_train_loss(const float* logits, const int64_t* x0, const int64_t* x_t, const int64_t* t, const float* pt, const float* sched,
                    float* dlogits, float* log_model_prob, float* col_loss, int* hits, float* kl_loss, float* vb_loss, float* loss,
                    float* lt_history, float* lt_count, float* scratch_b, int B, int K, int L, int T, float aux_weight, int adaptive,

@@ -65,6 +65,8 @@ SIGNATURES = {
     "dsb_attention_tc": [c_vp, c_ll, c_vp, c_ll, c_vp, c_ll, c_vp, c_ll, c_i, c_i, c_i, c_i, c_f, c_vp],
     "dsb_posterior_sample": [c_vp] * 8 + [c_i] * 5 + [c_f, c_i, c_i, c_vp],
     "dsb_posterior_sample_loop": [c_vp] * 8 + [c_i] * 5 + [c_f, c_i, c_vp],
+    "dsb_posterior_sample_wide": [c_vp] * 8 + [c_i] * 5 + [c_f, c_i, c_i, c_vp],
+    "dsb_posterior_sample_wide_loop": [c_vp] * 8 + [c_i] * 5 + [c_f, c_i, c_vp],
     "dsb_aten_uniform": [c_vp, c_ll, C.c_ulonglong, C.c_ulonglong, C.c_ulonglong, c_vp],
     # Melception feature extractor
     "dsb_mel_stem": [c_vp] * 5 + [c_f, c_vp] + [c_i] * 8 + [c_vp],

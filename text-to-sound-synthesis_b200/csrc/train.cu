@@ -5,6 +5,7 @@
 //              transformer_utils.py:43-58, :91-109 (attention), :111-115 (GELU2), :134-149 (AdaLayerNorm), :255-272 (Block);
 //              embeddings/dalle_mask_image_embedding.py:36-58.  The reference gets all of these gradients from torch autograd.
 // Activation storage type "T": float (tf32-rounded on store; DSB_DTYPE_TF32) or bf16 (DSB_DTYPE_BF16).
+#include "block_ctx.cuh"
 #include "common.cuh"
 #include "diffsound_b200.h"
 #include "train_loss_math.cuh"
@@ -136,6 +137,38 @@ train_loss_kernel(const float* __restrict__ logits, const int64_t* __restrict__ 
     col_out[2 * (long long)col] = o.main;
     col_out[2 * (long long)col + 1] = o.aux;
     if (hits) { hits[2 * (long long)col] = o.x0_hit; hits[2 * (long long)col + 1] = o.keep_hit; }
+  }
+}
+
+// Wide form for K + 1 > 32 * 33: one CTA of WIDE_LOSS_NT threads per column, CAP = ceil((K+1) / WIDE_LOSS_NT) values per thread, the
+// same column_loss on a block context (reductions in the fixed order of block_ctx.cuh).
+constexpr int WIDE_LOSS_NT = 256;
+constexpr int WIDE_LOSS_MAX_CAP = 16;  // K + 1 <= 4096
+
+template <int CAP>
+__global__ void __launch_bounds__(WIDE_LOSS_NT, CAP <= 9 ? 2 : 1)
+train_loss_wide_kernel(const float* __restrict__ logits, const int64_t* __restrict__ x0, const int64_t* __restrict__ xt,
+                       const int64_t* __restrict__ t, const float* __restrict__ pt, const float* __restrict__ sched, float* __restrict__ dlogits,
+                       float* __restrict__ prob_out, float* __restrict__ col_out, int* __restrict__ hits, int B, int K, int L, int T, float aux_w,
+                       int adaptive, float mw0, float mw1, int prob_exp) {
+  __shared__ double red[2 * (WIDE_LOSS_NT / 32)];
+  const long long col = blockIdx.x;
+  const int b = (int)(col / L), l = (int)(col - (long long)b * L);
+  const BlockCtx<WIDE_LOSS_NT> c{red, (int)threadIdx.x, 0};
+  const long long tb = t[b];
+  const dsb_loss::Sched s = dsb_loss::load_sched(sched, T, tb);
+  dsb_loss::ColumnIn in;
+  in.K = K; in.x0 = (int)x0[col]; in.xt = (int)xt[col]; in.is0 = tb == 0;
+  in.g_main = 1.f / (pt[b] * (float)(B * L));
+  in.g_aux = aux_w != 0.f ? in.g_main * aux_w * (adaptive ? ((float)tb / (float)T + 1.0f) : 1.0f) : 0.f;
+  in.mw0 = mw0; in.mw1 = mw1;
+  const dsb_loss::ColumnOut o = dsb_loss::column_loss<BlockCtx<WIDE_LOSS_NT>, CAP>(
+      c, logits + col * K, dlogits ? dlogits + col * K : nullptr,
+      prob_out ? prob_out + (long long)b * (K + 1) * L + l : nullptr, L, prob_exp != 0, in, s);
+  if (threadIdx.x == 0) {
+    col_out[2 * col] = o.main;
+    col_out[2 * col + 1] = o.aux;
+    if (hits) { hits[2 * col] = o.x0_hit; hits[2 * col + 1] = o.keep_hit; }
   }
 }
 
@@ -583,19 +616,27 @@ extern "C" int dsb_train_loss(const float* logits, const int64_t* x0, const int6
                               float* lt_history, float* lt_count, float* scratch_b, int B, int K, int L, int T, float aux_weight, int adaptive,
                               float mw0, float mw1, int prob_as_exp, void* stream) {
   DSB_REQUIRE(B > 0 && K > 0 && L > 0 && T > 0, "dsb_train_loss: bad shape");
-  DSB_REQUIRE(K + 1 <= 32 * 33, "dsb_train_loss: K=%d too large (max 1055)", K);
+  DSB_REQUIRE(K + 1 <= WIDE_LOSS_NT * WIDE_LOSS_MAX_CAP, "dsb_train_loss: K=%d too large (max %d)", K, WIDE_LOSS_NT * WIDE_LOSS_MAX_CAP - 1);
   DSB_REQUIRE(logits && x0 && x_t && t && pt && sched && col_loss && kl_loss && vb_loss && loss, "dsb_train_loss: null argument");
   DSB_REQUIRE(!lt_history || (lt_count && scratch_b), "dsb_train_loss: Lt bookkeeping needs lt_count and a B-float scratch");
   cudaStream_t st = (cudaStream_t)stream;
   const int nj = (K + 1 + 31) / 32;
   const int grid = (B * L + 7) / 8;
+  const int cap = (K + 1 + WIDE_LOSS_NT - 1) / WIDE_LOSS_NT;
 #define DSB_LOSS_CASE(N)                                                                                                               \
   if (nj <= N) {                                                                                                                       \
     train_loss_kernel<N><<<grid, 256, 0, st>>>(logits, x0, x_t, t, pt, sched, dlogits, log_model_prob, col_loss, hits, B, K, L, T,      \
                                                aux_weight, adaptive, mw0, mw1, prob_as_exp);                                           \
   } else
-  DSB_LOSS_CASE(2) DSB_LOSS_CASE(5) DSB_LOSS_CASE(9) DSB_LOSS_CASE(17) DSB_LOSS_CASE(33) { return 2; }
+#define DSB_WIDE_LOSS_CASE(N)                                                                                                          \
+  if (cap <= N) {                                                                                                                      \
+    train_loss_wide_kernel<N><<<B * L, WIDE_LOSS_NT, 0, st>>>(logits, x0, x_t, t, pt, sched, dlogits, log_model_prob, col_loss, hits, B, \
+                                                              K, L, T, aux_weight, adaptive, mw0, mw1, prob_as_exp);                   \
+  } else
+  DSB_LOSS_CASE(2) DSB_LOSS_CASE(5) DSB_LOSS_CASE(9) DSB_LOSS_CASE(17) DSB_LOSS_CASE(33)
+  DSB_WIDE_LOSS_CASE(9) DSB_WIDE_LOSS_CASE(WIDE_LOSS_MAX_CAP) { return 2; }
 #undef DSB_LOSS_CASE
+#undef DSB_WIDE_LOSS_CASE
   DSB_CHECK_CUDA(cudaGetLastError());
   train_loss_finalize_kernel<<<1, 256, 0, st>>>(col_loss, t, pt, kl_loss, vb_loss, loss, lt_history, lt_count, scratch_b, B, L, T, aux_weight, adaptive);
   DSB_CHECK_CUDA(cudaGetLastError());

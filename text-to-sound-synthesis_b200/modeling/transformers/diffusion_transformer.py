@@ -131,6 +131,12 @@ class DiffusionTransformer(nn.Module):
     def _trunc(self):
         return parse_truncation(self.truncation)
 
+    def _sampler_ops(self):
+        """(posterior_sample, posterior_sample_loop) for this codebook: one warp per column up to K = 1055, one CTA per column above."""
+        if self.num_classes - 1 > ops.WARP_SAMPLER_MAX_K:
+            return ops.posterior_sample_wide, ops.posterior_sample_wide_loop
+        return ops.posterior_sample, ops.posterior_sample_loop
+
     # ------------------------------------------------------------------ reference-compatible stage methods
     @torch.no_grad()
     def predict_start(self, log_x_t, cond_emb, t):
@@ -143,8 +149,8 @@ class DiffusionTransformer(nn.Module):
         B, L, K = blk.shape
         log_pred = torch.empty(B, K + 1, L, dtype=torch.float32, device=blk.device)
         mode, r, k = self._trunc()
-        ops.posterior_sample(blk, None, None, None, None, T=self.num_timesteps, trunc_mode=mode, trunc_r=r, trunc_k=k, log_prob_out=log_pred,
-                             stage=ops.STAGE_SKIP_POSTERIOR | ops.STAGE_SKIP_SAMPLE)
+        self._sampler_ops()[0](blk, None, None, None, None, T=self.num_timesteps, trunc_mode=mode, trunc_r=r, trunc_k=k, log_prob_out=log_pred,
+                               stage=ops.STAGE_SKIP_POSTERIOR | ops.STAGE_SKIP_SAMPLE)
         return log_pred
 
     @torch.no_grad()
@@ -153,16 +159,16 @@ class DiffusionTransformer(nn.Module):
         assert t.min().item() >= 0 and t.max().item() < self.num_timesteps
         x_t = log_x_t.argmax(1).contiguous()
         out = torch.empty_like(log_x_start, memory_format=torch.contiguous_format)
-        ops.posterior_sample(log_x_start.contiguous().float(), x_t, t.contiguous(), None, self._sched(), T=self.num_timesteps, trunc_mode=0,
-                             log_prob_out=out, stage=ops.STAGE_INPUT_LOGPROB | ops.STAGE_SKIP_SAMPLE)
+        self._sampler_ops()[0](log_x_start.contiguous().float(), x_t, t.contiguous(), None, self._sched(), T=self.num_timesteps, trunc_mode=0,
+                               log_prob_out=out, stage=ops.STAGE_INPUT_LOGPROB | ops.STAGE_SKIP_SAMPLE)
         return out
 
     @torch.no_grad()
     def log_sample_categorical(self, logits, return_index=False):
         """Gumbel-argmax with torch.rand_like's stream (diffusion_transformer.py:359-368); returns the log-one-hot re-encoding."""
         uniform = torch.rand_like(logits)
-        ids = ops.posterior_sample(logits.contiguous().float(), None, None, uniform, None, T=self.num_timesteps, trunc_mode=0,
-                                   stage=ops.STAGE_INPUT_LOGPROB | ops.STAGE_SKIP_POSTERIOR)
+        ids = self._sampler_ops()[0](logits.contiguous().float(), None, None, uniform, None, T=self.num_timesteps, trunc_mode=0,
+                                     stage=ops.STAGE_INPUT_LOGPROB | ops.STAGE_SKIP_POSTERIOR)
         return ids if return_index else index_to_log_onehot(ids, self.num_classes)
 
     def p_pred(self, log_x, cond_emb, t):
@@ -229,8 +235,8 @@ class DiffusionTransformer(nn.Module):
         eng = self.transformer.engine
         logits = eng.forward(st["x"], st["kv"], st["t"], st["Lc"])
         mode, r, k = st["trunc"]
-        ops.posterior_sample_loop(logits, st["x"], st["t"], st["t_post"], self._sched(), st["ctrl"], st["t_sched"], st["tp_sched"], T=self.num_timesteps,
-                                  trunc_mode=mode, trunc_r=r, trunc_k=k)
+        self._sampler_ops()[1](logits, st["x"], st["t"], st["t_post"], self._sched(), st["ctrl"], st["t_sched"], st["tp_sched"], T=self.num_timesteps,
+                               trunc_mode=mode, trunc_r=r, trunc_k=k)
 
     def _arm_loop(self, st, steps, post_steps, seed, offset, counter_offset, nthreads):
         """(Re)load the device-side loop state: RNG (seed, offset), the timestep schedule, step 0's t / t_post.  One small H2D copy per sample()."""

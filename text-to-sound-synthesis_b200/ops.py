@@ -382,6 +382,22 @@ def posterior_sample(inp, x_t, t, uniform, sched, *, T, trunc_mode=1, trunc_r=0.
                      stage=0):
     """Fused p_sample tail (see dsb_posterior_sample).  inp: raw logits (B,L,K) fp32, or (B,K+1,L) log-probs with STAGE_INPUT_LOGPROB;
     x_t (B,L) int64; uniform (B,K+1,L); sched (8,T+1) -> x_next (B,L) int64 (None when sampling is skipped)."""
+    return _posterior_sample("dsb_posterior_sample", inp, x_t, t, uniform, sched, T, trunc_mode, trunc_r, trunc_k, t_post, x_next, log_prob_out, stage)
+
+
+def posterior_sample_wide(inp, x_t, t, uniform, sched, *, T, trunc_mode=1, trunc_r=0.85, trunc_k=0, t_post=None, x_next=None, log_prob_out=None,
+                          stage=0):
+    """posterior_sample for codebooks up to K = WIDE_SAMPLER_MAX_K, one CTA per column (see dsb_posterior_sample_wide)."""
+    return _posterior_sample("dsb_posterior_sample_wide", inp, x_t, t, uniform, sched, T, trunc_mode, trunc_r, trunc_k, t_post, x_next, log_prob_out,
+                             stage)
+
+
+# Largest K of the warp-per-column sampler (posterior_sample / posterior_sample_loop) and of the CTA-per-column one (the _wide pair).
+WARP_SAMPLER_MAX_K = 1055
+WIDE_SAMPLER_MAX_K = 4095
+
+
+def _posterior_sample(fn, inp, x_t, t, uniform, sched, T, trunc_mode, trunc_r, trunc_k, t_post, x_next, log_prob_out, stage):
     _need_cuda(inp, x_t, t, uniform, sched, log_prob_out)
     if stage & STAGE_INPUT_LOGPROB:
         B, C_, L = inp.shape
@@ -397,8 +413,8 @@ def posterior_sample(inp, x_t, t, uniform, sched, *, T, trunc_mode=1, trunc_r=0.
         raise RuntimeError("sched must be (8, T+1)")
     if not (stage & STAGE_SKIP_SAMPLE) and x_next is None:
         x_next = torch.empty((B, L), dtype=torch.int64, device=inp.device)
-    _lib.check(_lib.lib().dsb_posterior_sample(inp.data_ptr(), _ptr(x_t), _ptr(t), _ptr(t_post), _ptr(uniform), _ptr(sched), _ptr(x_next),
-                                               _ptr(log_prob_out), B, K, L, T, trunc_mode, trunc_r, trunc_k, stage, _stream()), "dsb_posterior_sample")
+    _lib.check(getattr(_lib.lib(), fn)(inp.data_ptr(), _ptr(x_t), _ptr(t), _ptr(t_post), _ptr(uniform), _ptr(sched), _ptr(x_next),
+                                       _ptr(log_prob_out), B, K, L, T, trunc_mode, trunc_r, trunc_k, stage, _stream()), fn)
     return x_next
 
 
@@ -422,11 +438,20 @@ def aten_uniform(numel: int, seed: int, offset: int, device=None) -> torch.Tenso
 def posterior_sample_loop(logits, x, t, t_post, sched, ctrl, t_sched, t_post_sched, *, T, trunc_mode=1, trunc_r=0.85, trunc_k=0):
     """One step of the fused sampling loop (see dsb_posterior_sample_loop): in-kernel uniforms, x updated in place, t / t_post / RNG offset advanced on
     the device by the kernel itself."""
+    return _posterior_sample_loop("dsb_posterior_sample_loop", logits, x, t, t_post, sched, ctrl, t_sched, t_post_sched, T, trunc_mode, trunc_r, trunc_k)
+
+
+def posterior_sample_wide_loop(logits, x, t, t_post, sched, ctrl, t_sched, t_post_sched, *, T, trunc_mode=1, trunc_r=0.85, trunc_k=0):
+    """posterior_sample_loop for codebooks up to K = WIDE_SAMPLER_MAX_K, one CTA per column (see dsb_posterior_sample_wide_loop)."""
+    return _posterior_sample_loop("dsb_posterior_sample_wide_loop", logits, x, t, t_post, sched, ctrl, t_sched, t_post_sched, T, trunc_mode, trunc_r,
+                                  trunc_k)
+
+
+def _posterior_sample_loop(fn, logits, x, t, t_post, sched, ctrl, t_sched, t_post_sched, T, trunc_mode, trunc_r, trunc_k):
     _need_cuda(logits, x, t, t_post, sched, ctrl, t_sched, t_post_sched)
     B, L, K = logits.shape
-    _lib.check(_lib.lib().dsb_posterior_sample_loop(logits.data_ptr(), x.data_ptr(), t.data_ptr(), t_post.data_ptr(), sched.data_ptr(), ctrl.data_ptr(),
-                                                    t_sched.data_ptr(), t_post_sched.data_ptr(), B, K, L, T, trunc_mode, trunc_r, trunc_k, _stream()),
-               "dsb_posterior_sample_loop")
+    _lib.check(getattr(_lib.lib(), fn)(logits.data_ptr(), x.data_ptr(), t.data_ptr(), t_post.data_ptr(), sched.data_ptr(), ctrl.data_ptr(),
+                                       t_sched.data_ptr(), t_post_sched.data_ptr(), B, K, L, T, trunc_mode, trunc_r, trunc_k, _stream()), fn)
     return x
 
 
