@@ -240,6 +240,45 @@ int dsb_posterior_sample_wide_loop(const float* logits, int64_t* x, int64_t* t, 
 /* out[i] = the i-th element torch.rand(n, device='cuda') would hold for generator state (seed, philox offset) with ATen's launch geometry
  * nthreads = 256 * min(SMs * (maxThreadsPerSM / 256), ceil(n / 256)); used by the tests to pin the replay against torch.rand itself. */
 int dsb_aten_uniform(float* out, long long n, unsigned long long seed, unsigned long long offset, unsigned long long nthreads, void* stream);
+/* out[i] = the i-th element torch.empty(n, device='cuda').exponential_() would hold for generator state (seed, philox offset): the same Philox
+ * stream and geometry as dsb_aten_uniform, curand's (0, 1] value u, then -__logf(u) with ATen's clamp near 1 (TransformationHelper.h exponential(),
+ * DistributionTemplates.h exponential_kernel).  The draw torch.multinomial(probs, 1) makes on CUDA. */
+int dsb_aten_exponential(float* out, long long n, unsigned long long seed, unsigned long long offset, unsigned long long nthreads, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * Autoregressive SpecVQGAN transformer, KV-cached decode (reference Codebook/specvqgan/modules/transformer/mingpt.py GPTFeats / GPT,
+ * Codebook/specvqgan/models/cond_transformer.py Net2NetTransformer.sample).  One position of B rows per launch sequence; the current position p
+ * and the RNG state live in a device loop-control block of 8 uint64 words, advanced by dsb_ar_sample's last CTA, so one captured step replays
+ * for every position:
+ *   [0] seed  [1] philox offset  [2] offset increment per sampled position (ATen's counter_offset(B * V))  [3] ATen's thread count (256 * grid)
+ *   [4] position p  [5] number of positions  [6] first position that samples  [7] CTA ticket (0)
+ * Every kernel is a no-op at p >= [5].  The GEMMs between them are dsb_gemm_ex split-fp16 calls and the LayerNorms dsb_layernorm, unchanged.
+ * ------------------------------------------------------------------------------------------------------------- */
+/* mingpt.py:167-176 + :276-293 (embedder output prepended, tok_emb lookup, + pos_emb[:, :t]) at one position:
+ * x[b, :] = (p < Tc ? cond[b, p, :] : tok_emb[ids[b * ids_ld + p - Tc], :]) + pos_emb[p, :]; cond (B, Tc, D) is the Conv1d(k=1) embedding.
+ * An id outside [0, V) sets *err_flag (nn.Embedding's index error) and reads row 0.  With Tc = 0 (GPT without a condition) cond may be NULL. */
+int dsb_ar_embed(const float* cond, const float* tok_emb, const float* pos_emb, const int64_t* ids, long long ids_ld, float* x,
+                 const unsigned long long* ctrl, int B, int Tc, int V, int D, int* err_flag, void* stream);
+/* CausalSelfAttention (mingpt.py:76-94) for the one query row of position p, per (b, head): copies K / V of row b of qkv (fp32 (B, 3D) =
+ * [Q | K | V], row stride ld_qkv) bit-exactly into k_cache / v_cache (fp32, row b at b * cache_ld, position j at + j * D), then attends over
+ * cache rows 0 ... p in fp32 FMA arithmetic with a fixed reduction order: s_j = (q . k_j, ascending d) * scale, softmax with expf, o = sum_j
+ * p_j v_j.  o is written as the fp16 (hi | lo) pair of the proj GEMM's A operand (hi at out[b * ld_out + c], lo lo_off halves further).
+ * head_dim must be 32 or 64 (refused otherwise); max_pos (the cache capacity, sizes shared memory) <= 512.  A position p >= max_pos writes and
+ * reads nothing. */
+int dsb_ar_attention(const float* qkv, long long ld_qkv, float* k_cache, float* v_cache, long long cache_ld, int max_pos, void* out, long long ld_out,
+                     long long lo_off, const unsigned long long* ctrl, int B, int H, int head_dim, float scale, void* stream);
+/* nn.GELU() (exact erf form, mingpt.py:104-109) between the MLP GEMMs: y = x * 0.5 * (1 + erff(x / sqrt(2))) of fp32 in (rows, C), written
+ * as the fp16 (hi | lo) pair (hi at out[r * ld_out + c], lo lo_off halves further). */
+int dsb_gelu_erf_split(const float* in, long long ld_in, void* out, long long ld_out, long long lo_off, int rows, int C, void* stream);
+/* One sampling step of Net2NetTransformer.sample (cond_transformer.py:118-122, :171-186), one CTA per row b, V <= 4096:
+ * logits / temperature (fp32 division); top_k (1 ... V; 0 = None): entries below the top_k-th largest value become -inf (ties kept), by a
+ * bisection over the value's order-preserving key; fp32 softmax in a fixed order; do_sample: argmax(p / q) with q the replayed
+ * exponential_(1) of the (B, V) tensor at the control block's RNG state (torch.multinomial(probs, 1)'s CUDA fast path), else argmax(p); ties
+ * go to the lowest index.  At p >= ctrl[6] the id is written to ids[b * ids_ld + p - Tc + 1]; the last CTA advances p and, when it sampled,
+ * the philox offset.  A NaN probability (NaN / inf logits, all entries -inf) sets *err_flag.  Optional: probs_out (B, V) and logits_hist
+ * (raw logits of row b at position p written to logits_hist[b * hist_ld + p * V + k]). */
+int dsb_ar_sample(const float* logits, long long ld_logits, int64_t* ids, long long ids_ld, unsigned long long* ctrl, int B, int V, int Tc,
+                  float temperature, int top_k, int do_sample, float* probs_out, float* logits_hist, long long hist_ld, int* err_flag, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * SpecVQGAN decoder support (reference Diffsound/specvqgan/modules/diffusionmodules/model.py:570-671 Decoder and its

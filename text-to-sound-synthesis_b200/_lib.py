@@ -68,6 +68,12 @@ SIGNATURES = {
     "dsb_posterior_sample_wide": [c_vp] * 8 + [c_i] * 5 + [c_f, c_i, c_i, c_vp],
     "dsb_posterior_sample_wide_loop": [c_vp] * 8 + [c_i] * 5 + [c_f, c_i, c_vp],
     "dsb_aten_uniform": [c_vp, c_ll, C.c_ulonglong, C.c_ulonglong, C.c_ulonglong, c_vp],
+    "dsb_aten_exponential": [c_vp, c_ll, C.c_ulonglong, C.c_ulonglong, C.c_ulonglong, c_vp],
+    # autoregressive transformer decode
+    "dsb_ar_embed": [c_vp] * 4 + [c_ll, c_vp, c_vp] + [c_i] * 4 + [c_vp, c_vp],
+    "dsb_ar_attention": [c_vp, c_ll, c_vp, c_vp, c_ll, c_i, c_vp, c_ll, c_ll, c_vp, c_i, c_i, c_i, c_f, c_vp],
+    "dsb_gelu_erf_split": [c_vp, c_ll, c_vp, c_ll, c_ll, c_i, c_i, c_vp],
+    "dsb_ar_sample": [c_vp, c_ll, c_vp, c_ll, c_vp, c_i, c_i, c_i, c_f, c_i, c_i, c_vp, c_vp, c_ll, c_vp, c_vp],
     # Melception feature extractor
     "dsb_mel_stem": [c_vp] * 5 + [c_f, c_vp] + [c_i] * 8 + [c_vp],
     "dsb_pair_space_to_depth": [c_vp] + [c_i] * 6 + [c_vp] + [c_i] * 6 + [c_vp],

@@ -1,0 +1,223 @@
+"""Decode engine of the autoregressive SpecVQGAN transformer (Codebook/specvqgan/modules/transformer/mingpt.py GPTFeats / GPT): packs a
+drop-in GPT's parameters for the sm_90a kernels and runs the model one position at a time with a per-layer fp32 KV cache.
+
+The reference's Net2NetTransformer.sample (cond_transformer.py:124-194) re-runs the whole prefix for every token; because of the causal mask
+the last row of that forward only needs the keys and values of the earlier positions, so caching them computes the same logits in exact
+arithmetic.  One position of B rows is a fixed launch sequence (dsb_ar_* in include/diffsound_b200.h, GEMMs through ops.gemm_f16x3 with M = B):
+
+    embed, n_layer x [LayerNorm, QKV, decode attention, proj + residual, LayerNorm, MLP1, GELU(erf) + split, MLP2 + residual], ln_f, head, sampler
+
+The current position and the RNG state live in a device loop-control block that the sampler's last CTA advances, so the step is captured once as
+a CUDA graph and replayed for every position.  Teacher-forced forward() runs the same steps and records every position's logits.  One precision:
+every GEMM operand is an fp16 (hi | lo) pair ('f16x3', fp32-class results); the attention, softmax and sampler arithmetic is fp32.
+"""
+from __future__ import annotations
+
+import math
+from typing import Callable, Dict, Optional
+
+import numpy as np
+import torch
+
+from . import ops
+from .engine import _SplitWeight
+
+
+class AREngine:
+    def __init__(self, gpt, use_cuda_graph: bool = True):
+        self.m = gpt
+        self.use_cuda_graph = use_cuda_graph
+        self.packed = False
+        self._ws: Dict[int, dict] = {}
+        self.generation = 0  # bumped by repack(): graphs that baked old pointers are rebuilt
+        self._param_sig = None
+        self.launches_per_step = 0
+
+    def __deepcopy__(self, memo):
+        """copy.deepcopy(module) gets a fresh, unpacked engine bound to the copied module: packed weights, workspaces, KV caches and captured
+        graphs are per-instance caches, not state."""
+        return AREngine(memo.get(id(self.m), self.m), use_cuda_graph=self.use_cuda_graph)
+
+    def _signature(self):
+        """(storage pointer, in-place version counter) of every parameter: changes on optimizer.step(), p.data.copy_(), .to()."""
+        return tuple((p.data_ptr(), p._version) for p in self.m.parameters())
+
+    def ensure_current(self) -> None:
+        if not self.packed or self._param_sig != self._signature():
+            self.repack()
+
+    @property
+    def device(self):
+        return self.m.head.weight.device
+
+    @staticmethod
+    def _prep(w: torch.Tensor) -> _SplitWeight:
+        # (hi | lo) fp16 pair of 2^s * W with the largest weight near 2^13 (DenoiserEngine._prep); the GEMM epilogue multiplies by 2^-s
+        w = w.detach().float().contiguous()
+        amax = float(w.abs().max())
+        s = 0 if amax == 0.0 or not math.isfinite(amax) else 13 - math.frexp(amax)[1]
+        return _SplitWeight(ops.split_f16(w, 2.0 ** s), 2.0 ** (-s))
+
+    @torch.no_grad()
+    def repack(self) -> None:
+        """(Re)build packed copies from the module's current parameters."""
+        m = self.m
+        check_ar_shapes(m.config.vocab_size, m.config.n_embd, m.config.n_head, m.block_size)
+        if self.device.type != "cuda":
+            raise RuntimeError("AREngine needs the module on a CUDA device (no CPU fallback)")
+        f = lambda p: p.detach().float().contiguous()
+        self.D, self.H, self.V, self.P = m.config.n_embd, m.config.n_head, m.config.vocab_size, m.block_size
+        self.layers = []
+        for blk in m.blocks:
+            a = blk.attn
+            self.layers.append(dict(
+                g1=f(blk.ln1.weight), b1=f(blk.ln1.bias), eps1=blk.ln1.eps,
+                wqkv=self._prep(torch.cat([a.query.weight, a.key.weight, a.value.weight], 0)),
+                bqkv=f(torch.cat([a.query.bias, a.key.bias, a.value.bias], 0)),
+                wo=self._prep(a.proj.weight), bo=f(a.proj.bias),
+                g2=f(blk.ln2.weight), b2=f(blk.ln2.bias), eps2=blk.ln2.eps,
+                w1=self._prep(blk.mlp[0].weight), bm1=f(blk.mlp[0].bias),
+                w2=self._prep(blk.mlp[2].weight), bm2=f(blk.mlp[2].bias)))
+        self.gf, self.bf, self.epsf = f(m.ln_f.weight), f(m.ln_f.bias), m.ln_f.eps
+        self.whead = self._prep(m.head.weight)
+        self.tok_emb = f(m.tok_emb.weight)
+        self.pos_emb = f(m.pos_emb.reshape(m.pos_emb.shape[-2], m.pos_emb.shape[-1]))
+        emb = getattr(m, "embedder", None)
+        if emb is not None:
+            self.wc = f(emb.weight.reshape(emb.weight.shape[0], -1))
+            self.bc = f(emb.bias) if emb.bias is not None else None
+        self._param_sig = self._signature()
+        self.packed = True
+        self.generation += 1
+        self._ws.clear()
+
+    # ------------------------------------------------------------------ workspaces
+    def workspace(self, B: int) -> dict:
+        """Per-B buffers, sized for block_size positions: activations of one position, the per-layer fp32 K / V caches, the token ids, the
+        logits history, the loop-control block and the captured step graphs."""
+        ws = self._ws.get(B)
+        if ws is None:
+            dev, D, P, V = self.device, self.D, self.P, self.V
+            e = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+            pair = lambda r, c: torch.zeros(r, 2 * c, dtype=torch.float16, device=dev)
+            ws = dict(x=e(B, D), h=pair(B, D), qkv=e(B, 3 * D), att=pair(B, D), hid=e(B, 4 * D), hid2=pair(B, 4 * D), logits=e(B, V),
+                      kc=[torch.zeros(B, P, D, dtype=torch.float32, device=dev) for _ in self.layers],
+                      vc=[torch.zeros(B, P, D, dtype=torch.float32, device=dev) for _ in self.layers],
+                      cond=e(B * P * D), ids=torch.zeros(B, P + 1, dtype=torch.int64, device=dev), hist=None,
+                      ctrl=torch.zeros(ops.AR_CTRL_WORDS, dtype=torch.int64, device=dev),
+                      host=torch.zeros(ops.AR_CTRL_WORDS, dtype=torch.int64).pin_memory(),
+                      err=torch.zeros(2, dtype=torch.int32, device=dev), graphs={})
+            self._ws[B] = ws
+        return ws
+
+    # ------------------------------------------------------------------ compute
+    @torch.no_grad()
+    def embed_condition(self, feats: torch.Tensor) -> torch.Tensor:
+        """GPTFeats' Conv1d(Cf, D, 1) embedder (mingpt.py:286-289), once per call, in exact fp32: feats (B, Cf, Tc) -> (B, Tc, D)."""
+        self.ensure_current()
+        B, Cf, Tc = feats.shape
+        a = feats.detach().float().permute(0, 2, 1).reshape(B * Tc, Cf).contiguous()
+        return ops.gemm_f32(a, self.wc, self.bc).view(B, Tc, self.D)
+
+    def _step(self, ws, Tc: int, temperature: float, top_k: Optional[int], sample: bool, hist) -> None:
+        """One position: the fixed launch sequence (no host reads, capturable)."""
+        D, H = self.D, self.H
+        x, h, qkv, att, hid, hid2, ctrl = ws["x"], ws["h"], ws["qkv"], ws["att"], ws["hid"], ws["hid2"], ws["ctrl"]
+        B = x.shape[0]
+        cond = ws["cond"][:B * max(Tc, 1) * D].view(B, max(Tc, 1), D)[:, :Tc]
+        scale = 1.0 / math.sqrt(D // H)
+        ops.ar_embed(cond, self.tok_emb, self.pos_emb, ws["ids"], x, ctrl, err_flag=ws["err"][0:1])
+        for li, lay in enumerate(self.layers):
+            ops.layernorm(x, lay["g1"], lay["b1"], out=h, eps=lay["eps1"], split=True)
+            ops.gemm_f16x3(h, lay["wqkv"].pair, lay["bqkv"], out=qkv, alpha=lay["wqkv"].alpha)
+            ops.ar_attention(qkv, ws["kc"][li], ws["vc"][li], att, ctrl, H=H, scale=scale)
+            ops.gemm_f16x3(att, lay["wo"].pair, lay["bo"], residual=x, out=x, alpha=lay["wo"].alpha)
+            ops.layernorm(x, lay["g2"], lay["b2"], out=h, eps=lay["eps2"], split=True)
+            ops.gemm_f16x3(h, lay["w1"].pair, lay["bm1"], out=hid, alpha=lay["w1"].alpha)
+            ops.gelu_erf_split(hid, out=hid2)
+            ops.gemm_f16x3(hid2, lay["w2"].pair, lay["bm2"], residual=x, out=x, alpha=lay["w2"].alpha)
+        ops.layernorm(x, self.gf, self.bf, out=h, eps=self.epsf, split=True)
+        ops.gemm_f16x3(h, self.whead.pair, None, out=ws["logits"], alpha=self.whead.alpha)
+        ops.ar_sample(ws["logits"], ws["ids"], ctrl, Tc=Tc, temperature=temperature, top_k=top_k, sample=sample, logits_hist=hist,
+                      err_flag=ws["err"][1:2])
+        self.launches_per_step = 4 + 8 * len(self.layers)
+
+    def _arm(self, ws, seed, offset, counter_offset, nthreads, n_pos, first) -> None:
+        """(Re)load the device loop state: RNG (seed, offset), position 0, the number of positions and the first sampled one."""
+        c = ws["host"]
+        c[0] = np.array([seed & (2 ** 64 - 1)], dtype=np.uint64).view(np.int64)[0].item()
+        c[1], c[2], c[3], c[4], c[5], c[6], c[7] = offset, counter_offset, nthreads, 0, n_pos, first, 0
+        ws["ctrl"].copy_(c)  # blocking: the pinned staging buffer is rewritten by the next call
+
+    @torch.no_grad()
+    def run(self, cond: torch.Tensor, ids: torch.Tensor, n_pos: int, first: int, *, temperature: float = 1.0, top_k: Optional[int] = None,
+            sample: bool = False, record_logits: bool = False, callback: Optional[Callable[[int], None]] = None):
+        """Runs positions 0 ... n_pos - 1.  cond (B, Tc, D) fp32 (the embedded condition), ids (B, n) the given tokens; positions p >= first
+        write the token of position p + 1 (ids[b, p - Tc + 1]).  Returns (ids (B, n_pos - Tc + 1) when first < n_pos else None, logits history
+        (B, n_pos, V) when record_logits else None).  callback(k) runs on the host before the k-th sampled position."""
+        self.ensure_current()
+        B, Tc, _ = cond.shape
+        n_given = ids.shape[1]
+        dev = self.device
+        ws = self.workspace(B)
+        if Tc > 0:
+            ws["cond"][:B * Tc * self.D].view(B, Tc, self.D).copy_(cond)
+        hist = None
+        if record_logits:
+            if ws["hist"] is None:
+                ws["hist"] = torch.zeros(B, self.P, self.V, dtype=torch.float32, device=dev)
+            hist = ws["hist"]
+        gen = torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
+        seed, offset = gen.initial_seed(), gen.get_offset()
+        nthreads, counter_offset = ops.aten_rand_geometry(B * self.V, dev)
+        if n_given:  # before the capture warm-up below, which already embeds position 0 (a token when Tc = 0)
+            ws["ids"][:, :n_given].copy_(ids)
+        key = (Tc, float(temperature), top_k, bool(sample), record_logits)
+        g = ws["graphs"].get(key) if self.use_cuda_graph else None
+        if g is not None and g[1] != self.generation:
+            g = None
+        if self.use_cuda_graph and g is None:
+            # warm-up on a side stream (lazy inits), then capture one step; the loop state is re-armed afterwards
+            self._arm(ws, seed, offset, counter_offset, nthreads, n_pos, first)
+            s = torch.cuda.Stream(device=dev)
+            s.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(s):
+                self._step(ws, Tc, temperature, top_k, sample, hist)
+            torch.cuda.current_stream(dev).wait_stream(s)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                self._step(ws, Tc, temperature, top_k, sample, hist)
+            g = (graph, self.generation)
+            ws["graphs"][key] = g
+        self._arm(ws, seed, offset, counter_offset, nthreads, n_pos, first)
+        if n_given:  # the warm-up step may have written a sampled token over the given ones
+            ws["ids"][:, :n_given].copy_(ids)
+        for p in range(n_pos):
+            if callback is not None and p >= first:
+                callback(p - first)
+            if g is not None:
+                g[0].replay()
+            else:
+                self._step(ws, Tc, temperature, top_k, sample, hist)
+        n_sampled = max(0, n_pos - first)
+        if sample:
+            gen.set_offset(offset + n_sampled * counter_offset)
+        err = ws["err"].tolist()  # one 8-byte read per call
+        if any(err):
+            ws["err"].zero_()
+            if err[0]:
+                raise IndexError(f"index out of range in self: a token id >= vocab_size ({self.V}) reached GPT.tok_emb")
+            raise RuntimeError("probability tensor contains either `inf`, `nan` or element < 0")
+        out_ids = ws["ids"][:, :n_pos - Tc + 1].clone() if first < n_pos else None
+        out_hist = hist[:, :n_pos].clone() if record_logits else None
+        return out_ids, out_hist
+
+
+def check_ar_shapes(V: int, D: int, H: int, block_size: int) -> None:
+    """Refusals of the decode kernels, raised before anything is packed or launched."""
+    if V > ops.AR_MAX_V:
+        raise ValueError(f"vocab_size={V} too large: the autoregressive sampler takes at most {ops.AR_MAX_V} entries")
+    if D % H or D // H not in ops.AR_HEAD_DIMS:
+        raise ValueError(f"head_dim n_embd / n_head = {D}/{H} unsupported: the decode attention takes head_dim 32 or 64")
+    if block_size > ops.AR_MAX_POS:
+        raise ValueError(f"block_size={block_size} too large: the decode attention caches at most {ops.AR_MAX_POS} positions")

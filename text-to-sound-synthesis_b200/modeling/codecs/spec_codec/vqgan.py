@@ -28,6 +28,13 @@ class ColumnMajor(nn.Module):
         return x[:, self.backward_shuffle_idx] if reverse else x[:, self.forward_shuffle_idx]
 
 
+class Identity(nn.Module):
+    """permuter.py Identity: token order unchanged, no buffers."""
+
+    def forward(self, x, reverse=False):
+        return x
+
+
 class _Holder(nn.Module):
     def forward(self, *a, **k):
         raise RuntimeError(f"{type(self).__name__} only stores parameters; compute runs in DecoderEngine (CUDA kernels)")

@@ -600,3 +600,75 @@ def pair_channel_mean(x, window, *, inv_scale=1.0, out=None):
     _lib.check(_lib.lib().dsb_pair_channel_mean(x.data_ptr(), C2, C, Hp, Wp, *window, B, C, float(inv_scale), out.data_ptr(), _stream()),
                "dsb_pair_channel_mean")
     return out
+
+
+# ---------------------------------------------------------------- autoregressive transformer decode (ar_decode.cu)
+AR_MAX_V = 4096
+AR_HEAD_DIMS = (32, 64)
+AR_MAX_POS = 512
+AR_CTRL_WORDS = 8
+
+
+def aten_exponential(numel: int, seed: int, offset: int, device=None) -> torch.Tensor:
+    """The tensor torch.empty(numel, device='cuda').exponential_() would return for generator state (seed, philox offset), computed by this
+    library's Philox (the q that torch.multinomial(probs, 1) draws on CUDA)."""
+    out = torch.empty(numel, dtype=torch.float32, device=device if device is not None else "cuda")
+    nthreads, _ = aten_rand_geometry(numel, out.device)
+    _lib.check(_lib.lib().dsb_aten_exponential(out.data_ptr(), numel, seed & (2 ** 64 - 1), offset, nthreads, _stream()), "dsb_aten_exponential")
+    return out
+
+
+def ar_embed(cond, tok_emb, pos_emb, ids, x, ctrl, *, err_flag=None):
+    """x (B, D) = embedding of position ctrl[4]: cond (B, Tc, D) rows first, then tok_emb[ids (B, ids_ld)], plus pos_emb (P, D)."""
+    _need_cuda(cond, tok_emb, pos_emb, ids, x, ctrl, err_flag)
+    B, Tc, D = cond.shape
+    _lib.check(_lib.lib().dsb_ar_embed(cond.data_ptr(), tok_emb.data_ptr(), pos_emb.data_ptr(), ids.data_ptr(), ids.stride(0), x.data_ptr(), ctrl.data_ptr(),
+                                       B, Tc, tok_emb.shape[0], D, _ptr(err_flag), _stream()), "dsb_ar_embed")
+    return x
+
+
+def ar_attention(qkv, k_cache, v_cache, out, ctrl, *, H, scale, lo_off=None):
+    """Decode attention at position ctrl[4]: qkv (B, 3D) fp32 [Q | K | V]; k_cache / v_cache (B, P, D) fp32; out the fp16 (hi | lo) pair (B, 2D)."""
+    _need_cuda(qkv, k_cache, v_cache, out, ctrl)
+    B, P, D = k_cache.shape
+    if D % H or D // H not in AR_HEAD_DIMS:
+        raise ValueError(f"ar_attention: head_dim {D // H if D % H == 0 else D / H} unsupported (32 or 64)")
+    if P > AR_MAX_POS:
+        raise ValueError(f"ar_attention: {P} cache positions exceed {AR_MAX_POS}")
+    if out.dtype != torch.float16 or qkv.dtype != torch.float32 or k_cache.dtype != torch.float32 or not k_cache.is_contiguous() or not v_cache.is_contiguous():
+        raise RuntimeError("ar_attention: fp32 qkv and contiguous fp32 caches in, fp16 pair out")
+    _lib.check(_lib.lib().dsb_ar_attention(qkv.data_ptr(), qkv.stride(0), k_cache.data_ptr(), v_cache.data_ptr(), P * D, P, out.data_ptr(), out.stride(0),
+                                           D if lo_off is None else lo_off, ctrl.data_ptr(), B, H, D // H, float(scale), _stream()), "dsb_ar_attention")
+    return out
+
+
+def gelu_erf_split(x, out=None):
+    """nn.GELU() (exact erf) of fp32 x (rows, C), written as the fp16 (hi | lo) pair (rows, 2C)."""
+    _need_cuda(x, out)
+    rows, Cc = x.shape
+    if out is None:
+        out = torch.empty(rows, 2 * Cc, dtype=torch.float16, device=x.device)
+    _lib.check(_lib.lib().dsb_gelu_erf_split(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), Cc, rows, Cc, _stream()), "dsb_gelu_erf_split")
+    return out
+
+
+def ar_sample(logits, ids, ctrl, *, Tc, temperature=1.0, top_k=None, sample=True, probs_out=None, logits_hist=None, err_flag=None):
+    """One sampling step at position ctrl[4] (see dsb_ar_sample): logits (B, V) fp32 -> ids[b, p - Tc + 1] when p >= ctrl[6]; top_k None = no
+    truncation.  logits_hist (B, P, V) receives row p of the raw logits."""
+    _need_cuda(logits, ids, ctrl, probs_out, logits_hist, err_flag)
+    B, V = logits.shape
+    check_ar_sampler_args(V, top_k, temperature)
+    _lib.check(_lib.lib().dsb_ar_sample(logits.data_ptr(), logits.stride(0), ids.data_ptr(), ids.stride(0), ctrl.data_ptr(), B, V, Tc, float(temperature),
+                                        0 if top_k is None else int(top_k), 1 if sample else 0, _ptr(probs_out), _ptr(logits_hist),
+                                        0 if logits_hist is None else logits_hist.stride(0), _ptr(err_flag), _stream()), "dsb_ar_sample")
+    return ids
+
+
+def check_ar_sampler_args(V, top_k, temperature):
+    """The sampler's refusals, raised before anything is launched."""
+    if V > AR_MAX_V:
+        raise ValueError(f"the autoregressive sampler takes a vocabulary of at most {AR_MAX_V} entries, got {V}")
+    if top_k is not None and not 1 <= int(top_k) <= V:
+        raise ValueError(f"top_k={top_k} out of range: torch.topk needs 1 <= k <= vocab size ({V})")
+    if not float(temperature) == float(temperature) or float(temperature) == 0.0:
+        raise ValueError("temperature must be a non-zero number")

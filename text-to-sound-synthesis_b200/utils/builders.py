@@ -65,3 +65,31 @@ def build_vocoder(ckpt=None):
     if ckpt and os.path.exists(ckpt):
         voc.load_state_dict(torch.load(ckpt, map_location="cpu"), strict=True)
     return voc.cuda().eval()
+
+
+# the three autoregressive-transformer configs of Codebook/configs/ (caps_transformer.yaml, caps_transformer_2048.yaml,
+# caps_transformer_small.yaml): they differ only in vocab_size / n_layer / n_embd / n_head
+AR_CONFIGS = {"caps_transformer": dict(V=256, NL=19, D=1024, NH=16), "caps_transformer_2048": dict(V=2048, NL=19, D=1024, NH=16),
+              "caps_transformer_small": dict(V=256, NL=18, D=512, NH=16)}
+
+
+def ar_transformer_config(V=256, NL=19, D=1024, NH=16, Cf=512, block_size=266, ddconfig=None):
+    """`model` block of Codebook/configs/caps_transformer.yaml (reference class paths; retarget_config maps them to the drop-ins), without the
+    codebook checkpoint path."""
+    return {"target": "specvqgan.models.cond_transformer.Net2NetTransformer", "params": {
+        "cond_stage_key": "feature",
+        "transformer_config": {"target": "specvqgan.modules.transformer.mingpt.GPTFeats", "params": {
+            "feat_embedding_config": {"target": "torch.nn.Conv1d", "params": dict(in_channels=Cf, out_channels=D, kernel_size=1, padding=0)},
+            "GPT_config": dict(vocab_size=V, block_size=block_size, n_layer=NL, n_head=NH, n_embd=D)}},
+        "first_stage_permuter_config": {"target": "specvqgan.modules.transformer.permuter.ColumnMajor", "params": {"H": 5, "W": 53}},
+        "first_stage_config": {"target": "specvqgan.models.vqgan.VQModel", "params": {
+            "ckpt_path": None, "embed_dim": 256, "n_embed": V, "ddconfig": dict(ddconfig or DDCONFIG),
+            "lossconfig": {"target": "specvqgan.modules.losses.DummyLoss"}}},
+        "cond_stage_config": {"target": "specvqgan.modules.misc.raw_feats.RawFeatsStage"}}}
+
+
+def build_ar_transformer(config, seed=0, device="cuda"):
+    """Net2NetTransformer drop-in from a reference-style `model` config (e.g. ar_transformer_config(**AR_CONFIGS[name])), seeded random init
+    (the reference's own init order), eval mode, on `device`."""
+    torch.manual_seed(seed)
+    return instantiate_from_config(retarget_config(config)).to(device).eval()

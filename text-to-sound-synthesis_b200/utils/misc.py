@@ -34,6 +34,17 @@ TARGET_MAP = {
         "diffsound_b200.modeling.embeddings.clip_text_embedding.CLIPTextEmbedding",
     "sound_synthesis.engine.ema.EMA":
         "diffsound_b200.engine_utils.ema.EMA",
+    # the autoregressive SpecVQGAN baseline (Codebook/configs/caps_transformer*.yaml)
+    "specvqgan.models.cond_transformer.Net2NetTransformer":
+        "diffsound_b200.modeling.models.cond_transformer.Net2NetTransformer",
+    "specvqgan.modules.transformer.mingpt.GPTFeats":
+        "diffsound_b200.modeling.transformers.mingpt.GPTFeats",
+    "specvqgan.models.vqgan.VQModel":
+        "diffsound_b200.modeling.codecs.spec_codec.vqgan.VQModel",
+    "specvqgan.modules.misc.raw_feats.RawFeatsStage":
+        "diffsound_b200.modeling.modules.raw_feats.RawFeatsStage",
+    "specvqgan.modules.transformer.permuter.Identity":
+        "diffsound_b200.modeling.codecs.spec_codec.vqgan.Identity",
 }
 
 
