@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from . import ops
-from .engine import _SplitWeight
+from .packing import SplitWeight
 
 
 class AREngine:
@@ -50,14 +50,6 @@ class AREngine:
     def device(self):
         return self.m.head.weight.device
 
-    @staticmethod
-    def _prep(w: torch.Tensor) -> _SplitWeight:
-        # (hi | lo) fp16 pair of 2^s * W with the largest weight near 2^13 (DenoiserEngine._prep); the GEMM epilogue multiplies by 2^-s
-        w = w.detach().float().contiguous()
-        amax = float(w.abs().max())
-        s = 0 if amax == 0.0 or not math.isfinite(amax) else 13 - math.frexp(amax)[1]
-        return _SplitWeight(ops.split_f16(w, 2.0 ** s), 2.0 ** (-s))
-
     @torch.no_grad()
     def repack(self) -> None:
         """(Re)build packed copies from the module's current parameters."""
@@ -72,14 +64,14 @@ class AREngine:
             a = blk.attn
             self.layers.append(dict(
                 g1=f(blk.ln1.weight), b1=f(blk.ln1.bias), eps1=blk.ln1.eps,
-                wqkv=self._prep(torch.cat([a.query.weight, a.key.weight, a.value.weight], 0)),
+                wqkv=SplitWeight(torch.cat([a.query.weight, a.key.weight, a.value.weight], 0)),
                 bqkv=f(torch.cat([a.query.bias, a.key.bias, a.value.bias], 0)),
-                wo=self._prep(a.proj.weight), bo=f(a.proj.bias),
+                wo=SplitWeight(a.proj.weight), bo=f(a.proj.bias),
                 g2=f(blk.ln2.weight), b2=f(blk.ln2.bias), eps2=blk.ln2.eps,
-                w1=self._prep(blk.mlp[0].weight), bm1=f(blk.mlp[0].bias),
-                w2=self._prep(blk.mlp[2].weight), bm2=f(blk.mlp[2].bias)))
+                w1=SplitWeight(blk.mlp[0].weight), bm1=f(blk.mlp[0].bias),
+                w2=SplitWeight(blk.mlp[2].weight), bm2=f(blk.mlp[2].bias)))
         self.gf, self.bf, self.epsf = f(m.ln_f.weight), f(m.ln_f.bias), m.ln_f.eps
-        self.whead = self._prep(m.head.weight)
+        self.whead = SplitWeight(m.head.weight)
         self.tok_emb = f(m.tok_emb.weight)
         self.pos_emb = f(m.pos_emb.reshape(m.pos_emb.shape[-2], m.pos_emb.shape[-1]))
         emb = getattr(m, "embedder", None)

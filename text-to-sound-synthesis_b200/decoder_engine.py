@@ -96,11 +96,10 @@ class DecoderEngine:
         Cin, R, N = C2 // 2, B * Hp * Wp, cv.N
         shifts = [dy * Wp + dx for dy in (-1, 0, 1) for dx in (-1, 0, 1)] if k == 3 else [0]
         out = torch.empty(B, Hp, Wp, 2 * N if pair_out else N, dtype=torch.float16 if pair_out else torch.float32, device=x.device)
-        ops.gemm_desc(A=x.data_ptr(), W=cv.w.data_ptr(), out=out.data_ptr(), M=R, N=N, K=cv.Kp, taps=cv.taps([(sh, 0, Cin, 0) for sh in shifts]),
-                      a_rows=R, a_cols=C2, lda=C2, ldw=cv.w.shape[1], w_cols=cv.w.shape[1], ldo=out.shape[-1], bias=cv.bias, alpha=cv.alpha,
-                      flags=ops.OUT_F16_SPLIT if pair_out else 0, split_off=N if pair_out else 0,
-                      residual=None if residual is None else residual.data_ptr(), ld_res=0 if residual is None else residual.shape[-1],
-                      geo=(Hp * Wp, Wp, 1, Hp - 1, 1, Wp - 1))
+        cv.launch(A=x.data_ptr(), out=out.data_ptr(), M=R, taps=cv.taps([(sh, 0, Cin, 0) for sh in shifts]), a_rows=R, a_cols=C2, lda=C2,
+                  ldo=out.shape[-1], bias=cv.bias, flags=ops.OUT_F16_SPLIT if pair_out else 0, split_off=N if pair_out else 0,
+                  residual=None if residual is None else residual.data_ptr(), ld_res=0 if residual is None else residual.shape[-1],
+                  geo=(Hp * Wp, Wp, 1, Hp - 1, 1, Wp - 1))
         self.launches += 1
         return out
 

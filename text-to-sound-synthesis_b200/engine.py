@@ -17,6 +17,7 @@ from typing import Dict, Optional
 import torch
 
 from . import ops
+from .packing import SplitWeight
 
 
 class DenoiserEngine:
@@ -61,11 +62,7 @@ class DenoiserEngine:
     def _prep(self, w: torch.Tensor):
         w = w.detach().float().contiguous()
         if self.precision == "f16x3":
-            # (hi | lo) fp16 pair of 2^s * W, s chosen so the largest weight sits near 2^13: the lo halves of ordinary weights stay
-            # clear of fp16's subnormal range; the GEMM epilogue multiplies by alpha = 2^-s (exact)
-            amax = float(w.abs().max())
-            s = 0 if amax == 0.0 or not math.isfinite(amax) else 13 - math.frexp(amax)[1]
-            return _SplitWeight(ops.split_f16(w, 2.0 ** s), 2.0 ** (-s))
+            return SplitWeight(w)
         if self.precision == "f16":
             return ops.to_f16(w)
         return ops.round_tf32(w) if self.precision == "tf32" else w.clone()
@@ -251,14 +248,3 @@ class DenoiserEngine:
         self.launches_per_forward = n + 2
         return logits
 
-
-class _SplitWeight:
-    """fp16 (hi | lo) pair of 2^s * W, (N, 2K), plus alpha = 2^-s for the GEMM epilogue."""
-    __slots__ = ("pair", "alpha")
-
-    def __init__(self, pair, alpha):
-        self.pair, self.alpha = pair, alpha
-
-    @property
-    def shape(self):
-        return (self.pair.shape[0], self.pair.shape[1] // 2)

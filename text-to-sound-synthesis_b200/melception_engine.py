@@ -25,13 +25,11 @@ Reference: Codebook/evaluation/feature_extractors/melception.py:23-113, torchvis
 """
 from __future__ import annotations
 
-import math
-
 import torch
 
 from . import ops
 from .graphs import GraphCache
-from .packing import PackedConv
+from .packing import PackedConv, activation_scale
 
 FEATURES = ("64", "192", "768", "2048", "logits_unbiased", "logits")
 _DEPTH = {"64": 0, "192": 1, "768": 2, "2048": 3, "logits_unbiased": 3, "logits": 3}
@@ -128,16 +126,14 @@ class MelceptionEngine:
     # ------------------------------------------------------------------------------------------------ producers of one stored tensor
     def _produce(self, key, prods, calibrate, extra_amax=0.0):
         """Run the launches `prods` that together write the tensor `key`; each is prod(measure): measure=True runs it unscaled with its last
-        launch NO_STORE into self._amax.  Calibration measures first and sets sigma[key] so the largest magnitude lands in (2^8, 2^9]."""
+        launch NO_STORE into self._amax.  Calibration measures first and sets sigma[key] = packing.activation_scale of the largest magnitude."""
         if calibrate:
             self._amax.zero_()
             for p in prods:
                 p(True)
             m = max(float(self._amax.item()), extra_amax)
-            if not (m > 0.0 and math.isfinite(m)):
-                raise RuntimeError(f"Melception calibration: tensor {key} has amax = {m} (non-finite weights or an all-zero activation)")
+            self.sig[key] = activation_scale(m, f"Melception calibration: tensor {key}")
             self.amax[key] = m
-            self.sig[key] = 2.0 ** (9 - math.ceil(math.log2(m)))
         for p in prods:
             p(False)
 
@@ -167,27 +163,27 @@ class MelceptionEngine:
         taps = cv.taps(sp)
         y0, x0, H, W = win
         geo = (Hp * Wp, Wp, y0, y0 + H, x0, x0 + W)
-        common = dict(A=A.data_ptr(), W=cv.w.data_ptr(), M=M, N=cv.N, K=cv.Kp, a_rows=M, a_cols=lda, lda=lda, ldw=cv.w.shape[1], w_cols=cv.w.shape[1])
+        common = dict(A=A.data_ptr(), M=M, a_rows=M, a_cols=lda, lda=lda)
         optr = out.data_ptr() + 2 * off
         SPLIT, RELU = ops.OUT_F16_SPLIT, ops.RELU
         sig_in = self.sig[x.key]
 
         def run(measure):
             so = 1.0 if measure else self.sig[key]
-            alpha = cv.alpha * so / sig_in
+            alpha = so / sig_in
             bias = self._bias_for(name, key, measure)
             last = dict(out=optr, ldo=C2o, split_off=Ctot, flags=SPLIT | RELU | (ops.NO_STORE if measure else 0), geo=geo,
                         amax_out=self._amax if measure else None)
             if len(taps) <= 32:
-                ops.gemm_desc(**common, taps=taps, bias=bias, alpha=alpha, **last)
+                cv.launch(**common, taps=taps, bias=bias, alpha=alpha, **last)
                 return
             # 5x5: 25 spatial taps = 75 entries -> 27 + 24 + 24, the fp32 partial sum chained through `residual` in place
             part = torch.empty(M, cv.N, dtype=torch.float32, device=out.device)
             chunks = [taps[:27], taps[27:51], taps[51:]]
-            ops.gemm_desc(**common, taps=chunks[0], alpha=alpha, out=part.data_ptr(), ldo=cv.N, flags=0)
-            ops.gemm_desc(**common, taps=chunks[1], alpha=alpha, out=part.data_ptr(), ldo=cv.N, flags=0, residual=part.data_ptr(), ld_res=cv.N)
+            cv.launch(**common, taps=chunks[0], alpha=alpha, out=part.data_ptr(), ldo=cv.N, flags=0)
+            cv.launch(**common, taps=chunks[1], alpha=alpha, out=part.data_ptr(), ldo=cv.N, flags=0, residual=part.data_ptr(), ld_res=cv.N)
             last["flags"] |= ops.RES_BEFORE_ACT
-            ops.gemm_desc(**common, taps=chunks[2], alpha=alpha, bias=bias, residual=part.data_ptr(), ld_res=cv.N, **last)
+            cv.launch(**common, taps=chunks[2], alpha=alpha, bias=bias, residual=part.data_ptr(), ld_res=cv.N, **last)
         return run
 
     def _conv(self, name, x, win, calibrate, *, phases=None):
@@ -296,9 +292,7 @@ class MelceptionEngine:
             tmp = torch.empty_like(t0)
             ops.mel_stem(x, w0, b0, tmp, Hp=Hp, Wp=Wp, y0=1, x0=1, scale=1.0)
             m = float(tmp.float().abs().max())
-            if not (m > 0.0 and math.isfinite(m)):
-                raise RuntimeError(f"Melception calibration: the stem's amax is {m}")
-            self.amax[key], self.sig[key] = m, 2.0 ** (9 - math.ceil(math.log2(m)))
+            self.amax[key], self.sig[key] = m, activation_scale(m, "Melception calibration: the stem")
         ops.mel_stem(x, w0, b0, t0, Hp=Hp, Wp=Wp, y0=1, x0=1, scale=self.sig[key], mean=self.mean, std=self.std)
         h = _Act(t0, w0.shape[0], key, (1, 1, H1, W1))
         h = self._conv("Conv2d_2a_3x3", h, (2, 2, H1 - 2, W1 - 2), calibrate)

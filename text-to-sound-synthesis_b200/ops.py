@@ -129,8 +129,20 @@ def gemm_f16x3(a_pair: torch.Tensor, w_pair: torch.Tensor, bias=None, residual=N
     M = a_pair.shape[0]
     if out is None:
         out = torch.empty(M, 2 * N, dtype=torch.float16, device=a_pair.device) if split_out else torch.empty(M, N, dtype=torch.float32, device=a_pair.device)
-    return gemm(a_pair, w_pair, bias, residual, out, dtype=F16, taps=[0, 0, 0], tap_acol=[K, 0, 0], tap_wcol=[0, K, 0], k_per_tap=K, alpha=alpha,
+    shifts, acols, wcols, _ = zip(*f16x3_taps([(0, 0, K, 0)], [(0, K)]))
+    return gemm(a_pair, w_pair, bias, residual, out, dtype=F16, taps=shifts, tap_acol=acols, tap_wcol=wcols, k_per_tap=K, alpha=alpha,
                 gelu=gelu, split_out=split_out, **kw)
+
+
+def f16x3_taps(spatial, w_cols):
+    """The split-fp16 tap list: per K-block j, spatial[j] = (row_shift, A hi column, A lo column, use_a2) and w_cols[j] = (W hi column, W lo column)
+    -> the triple (A lo . W hi), (A hi . W lo), (A hi . W hi) as (row_shift, a_col, w_col, use_a2) entries.  dsb_gemm_ex recognises exactly this
+    form (same shift within a triple, constant hi -> lo distances) and runs the three products off one staged copy of the operands with a per-k-block
+    fp32 promotion; any other list takes the plain tap loop, which is slower and rounds differently."""
+    out = []
+    for (sh, ah, al, a2), (wh, wl) in zip(spatial, w_cols):
+        out += [(sh, al, wh, a2), (sh, ah, wl, a2), (sh, ah, wh, a2)]
+    return out
 
 
 def silu(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -170,37 +182,16 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
     out_bf16 = out.dtype == torch.bfloat16
     if split_out and (out.dtype != torch.float16 or batched):
         raise RuntimeError("gemm: split_out writes an fp16 (hi | lo) pair and is not batched")
-    d = _lib.GemmDesc()
-    d.A, d.W, d.bias, d.residual, d.out = a.data_ptr(), w.data_ptr(), _ptr(bias), _ptr(residual), out.data_ptr()
-    d.M, d.N, d.K, d.batch = M, N, K, batch
-    d.a_rows = a_rows
-    d.lda, d.ldw, d.ldo = a.stride(-2), w.stride(-2), out.stride(-2)
-    d.ld_res = residual.stride(-2) if residual is not None else 0
-    d.a_batch_stride = a.stride(0) if batched else 0
-    d.w_batch_stride = w.stride(0) if w.dim() == 3 else 0
-    d.out_batch_stride = out.stride(0) if batched else 0
-    d.res_batch_stride = residual.stride(0) if (residual is not None and batched) else 0
-    d.dtype = dtype
-    d.flags = (GELU2 if gelu else 0) | (ROUND_TF32 if round_out else 0) | (OUT_BF16 if out_bf16 else 0) | (LRELU if lrelu else 0) | (TANH if tanh else 0) | (RELU if relu else 0) | (RES_BEFORE_ACT if res_before_act else 0) | (OUT_F16 if out_f16 else 0) | (OUT_F16_SPLIT if split_out else 0)
-    if split_out:
-        d.split_off = N
-    if tap_wcol is not None:
-        d.use_tap_wcol = 1
-        d.w_cols = w.shape[-1]
-        for i, c_ in enumerate(tap_wcol):
-            d.tap_wcol[i] = int(c_)
-    d.num_taps = ntaps
-    for i, s in enumerate(taps or [0]):
-        d.tap_shift[i] = int(s)
-        d.tap_acol[i] = int(tap_acol[i]) if tap_acol is not None else 0
-    d.a_cols = a_cols
-    if geo is not None:
-        d.geo_P, d.geo_Wp, d.geo_y0, d.geo_y1, d.geo_x0, d.geo_x1 = [int(v) for v in geo]
-    d.alpha = alpha
-    d.block_n, d.max_ctas, d.cta_pair = block_n, max_ctas, cta_pair
-    d.a_mn_major, d.b_mn_major = int(a_mn), int(w_mn)
-    d.schedule = schedule
-    _lib.check(_lib.lib().dsb_gemm_ex(C.byref(d), _stream()), "dsb_gemm_ex")
+    flags = (GELU2 if gelu else 0) | (ROUND_TF32 if round_out else 0) | (OUT_BF16 if out_bf16 else 0) | (LRELU if lrelu else 0) | (TANH if tanh else 0) | (RELU if relu else 0) | (RES_BEFORE_ACT if res_before_act else 0) | (OUT_F16 if out_f16 else 0) | (OUT_F16_SPLIT if split_out else 0)
+    shifts = taps or [0]
+    _gemm_ex([(s, tap_acol[i] if tap_acol is not None else 0, tap_wcol[i] if tap_wcol is not None else 0, 0) for i, s in enumerate(shifts)],
+             geo, use_tap_wcol=int(tap_wcol is not None), num_taps=ntaps,
+             A=a.data_ptr(), W=w.data_ptr(), bias=_ptr(bias), residual=_ptr(residual), out=out.data_ptr(), M=M, N=N, K=K, batch=batch,
+             a_rows=a_rows, a_cols=a_cols, lda=a.stride(-2), ldw=w.stride(-2), ldo=out.stride(-2), ld_res=residual.stride(-2) if residual is not None else 0,
+             a_batch_stride=a.stride(0) if batched else 0, w_batch_stride=w.stride(0) if w.dim() == 3 else 0,
+             out_batch_stride=out.stride(0) if batched else 0, res_batch_stride=residual.stride(0) if (residual is not None and batched) else 0,
+             dtype=dtype, flags=flags, split_off=N if split_out else 0, w_cols=w.shape[-1] if tap_wcol is not None else 0, alpha=alpha,
+             block_n=block_n, max_ctas=max_ctas, cta_pair=cta_pair, a_mn_major=int(a_mn), b_mn_major=int(w_mn), schedule=schedule)
     return out
 
 
@@ -210,23 +201,27 @@ def gemm_desc(*, A, W, out, M, N, K, taps, lda, ldw, ldo, dtype=F16, batch=1, a_
               schedule=0):
     """Thin front end of dsb_gemm_ex for callers that lay out their own buffers (the MelGAN / SpecVQGAN state buffers): A / W / out / A2 are
     raw device addresses (ints: tensor.data_ptr() plus a byte offset), sizes and strides in elements; taps = [(row_shift, a_col, w_col, use_a2), ...]."""
+    _gemm_ex(taps, geo, use_tap_wcol=1, num_taps=len(taps), A=A, W=W, out=out, bias=_ptr(bias), A2=A2, M=M, N=N, K=K, batch=batch,
+             a_rows=a_rows, a_cols=a_cols, lda=lda, ldw=ldw, ldo=ldo, a_batch_stride=a_batch_stride, out_batch_stride=out_batch_stride,
+             dtype=dtype, flags=flags, alpha=alpha, w_cols=w_cols, split_off=split_off, dual_off=dual_off, out_col_group=out_col_group,
+             out_col_group_stride=out_col_group_stride, lda2=lda2, a2_rows=a2_rows, a2_cols=a2_cols, a2_batch_stride=a2_batch_stride,
+             block_n=block_n, cta_pair=cta_pair, residual=residual, ld_res=ld_res, amax_out=_ptr(amax_out), resident_w=int(resident_w),
+             schedule=schedule)
+
+
+_DESC_FIELDS = frozenset(name for name, _ in _lib.GemmDesc._fields_)
+
+
+def _gemm_ex(taps, geo, **fields):
+    """Fill one GemmDesc and launch dsb_gemm_ex: `fields` are GemmDesc members by name (pointers as ints or None), taps = [(row_shift, a_col,
+    w_col, use_a2), ...], geo = (P, Wp, y0, y1, x0, x1) or None; every member not given stays zero."""
     d = _lib.GemmDesc()
-    d.A, d.W, d.out, d.bias, d.A2 = A, W, out, _ptr(bias), A2
-    d.M, d.N, d.K, d.batch = M, N, K, batch
-    d.a_rows, d.a_cols, d.lda, d.ldw, d.ldo = a_rows, a_cols, lda, ldw, ldo
-    d.a_batch_stride, d.out_batch_stride = a_batch_stride, out_batch_stride
-    d.dtype, d.flags, d.alpha = dtype, flags, alpha
-    d.num_taps = len(taps)
-    d.use_tap_wcol, d.w_cols = 1, w_cols
+    for name, v in fields.items():
+        if name not in _DESC_FIELDS:  # a ctypes Structure would silently keep a misspelt name as a plain attribute
+            raise TypeError(f"GemmDesc has no member {name!r}")
+        setattr(d, name, v)
     for i, (sh, ac, wc, a2) in enumerate(taps):
         d.tap_shift[i], d.tap_acol[i], d.tap_wcol[i], d.tap_a2[i] = int(sh), int(ac), int(wc), int(a2)
-    d.split_off, d.dual_off, d.out_col_group, d.out_col_group_stride = split_off, dual_off, out_col_group, out_col_group_stride
-    d.lda2, d.a2_rows, d.a2_cols, d.a2_batch_stride = lda2, a2_rows, a2_cols, a2_batch_stride
-    d.block_n, d.cta_pair = block_n, cta_pair
-    d.residual, d.ld_res = residual, ld_res
-    d.amax_out = _ptr(amax_out)
-    d.resident_w = int(resident_w)
-    d.schedule = schedule
     if geo is not None:
         d.geo_P, d.geo_Wp, d.geo_y0, d.geo_y1, d.geo_x0, d.geo_x1 = [int(v) for v in geo]
     _lib.check(_lib.lib().dsb_gemm_ex(C.byref(d), _stream()), "dsb_gemm_ex")

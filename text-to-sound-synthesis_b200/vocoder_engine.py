@@ -27,13 +27,11 @@ Reference: vocoder/modules.py:72-85 (ResnetBlock), :88-130 (Generator).
 """
 from __future__ import annotations
 
-import math
-
 import torch
 
 from . import ops
 from .graphs import GraphCache
-from .packing import PackedConv as _PackedConv
+from .packing import PackedConv as _PackedConv, activation_scale
 
 P = 9  # pad rows on either side of every clip in a state buffer (largest dilation / half kernel)
 
@@ -143,32 +141,19 @@ class VocoderEngine:
         return self._forward(mel)
 
     def _scaled(self, key, sig_in, calibrate, calls):
-        """Launch the GEMM(s) `calls` = [(PackedConv, kwargs)] that together produce ONE stored tensor; returns that tensor's scale sigma_out.
-        stored_out = sigma_out * (alpha_w / sigma_in * (A_stored . W_packed) + bias).  Calibration: a NO_STORE pass measures the largest true
-        magnitude, sigma_out = the power of two that maps it into (2^8, 2^9]."""
+        """Launch the GEMM(s) `calls` = [(PackedConv, PackedConv.launch kwargs)] that together produce ONE stored tensor; returns that tensor's
+        scale sigma_out.  stored_out = sigma_out * (alpha_w / sigma_in * (A_stored . W_packed) + bias).  Calibration: a NO_STORE pass measures the
+        largest true magnitude, sigma_out = packing.activation_scale of it."""
         if calibrate:
             self._amax.zero_()
             for cv, kw in calls:
-                ops.gemm_desc(**dict(kw, flags=kw["flags"] | ops.NO_STORE), W=cv.w.data_ptr(), ldw=cv.w.shape[1], w_cols=cv.w.shape[1],
-                              K=64 if kw.get("resident_w") else cv.Kp, alpha=cv.alpha / sig_in, bias=cv.bias, amax_out=self._amax)
-            m = float(self._amax.item())
-            if not (m > 0.0 and math.isfinite(m)):
-                raise RuntimeError(f"MelGAN calibration: launch site {key} produced amax = {m}")
-            self.sig[key] = 2.0 ** (9 - math.ceil(math.log2(m)))
+                cv.launch(**dict(kw, flags=kw["flags"] | ops.NO_STORE), alpha=1.0 / sig_in, bias=cv.bias, amax_out=self._amax)
+            self.sig[key] = activation_scale(float(self._amax.item()), f"MelGAN calibration: launch site {key}")
             self.bias_s[key] = [(cv.bias * self.sig[key]).contiguous() for cv, _ in calls]
         so = self.sig[key]
         for (cv, kw), bs in zip(calls, self.bias_s[key]):
-            ops.gemm_desc(**kw, W=cv.w.data_ptr(), ldw=cv.w.shape[1], w_cols=cv.w.shape[1], K=64 if kw.get("resident_w") else cv.Kp,
-                          alpha=cv.alpha * so / sig_in, bias=bs)
+            cv.launch(**kw, alpha=so / sig_in, bias=bs)
         return so
-
-    @staticmethod
-    def _taps(cv, spatial):
-        """(tap list, resident_w): narrow layers (N <= 128, at most 96 KB of weights, packing.resident_ok) run as 64-deep taps (dsb_gemm_ex resident_w form)."""
-        t64 = cv.taps64(spatial)
-        if cv.resident_ok(len(t64)):
-            return dict(taps=t64, resident_w=1)
-        return dict(taps=cv.taps(spatial), resident_w=0)
 
     def _forward(self, mel: torch.Tensor, calibrate: bool = False) -> torch.Tensor:
         B, Cm, T = mel.shape
@@ -183,7 +168,7 @@ class VocoderEngine:
         S, C = states[0], self.c0
         Cs = _c8(C)
         sig = self._scaled("first", 1.0, calibrate, [(cv, dict(
-            A=mp.data_ptr(), out=S.data_ptr() + 2 * (P * 4 * Cs + 2 * Cs), M=T, N=C, batch=B, taps=cv.taps([(j, 0, cv.Kp, 0) for j in range(7)]),
+            A=mp.data_ptr(), out=S.data_ptr() + 2 * (P * 4 * Cs + 2 * Cs), M=T, batch=B, taps=cv.taps([(j, 0, cv.Kp, 0) for j in range(7)]),
             a_rows=T + 6, a_cols=2 * cv.Kp, lda=2 * cv.Kp, a_batch_stride=(T + 6) * 2 * cv.Kp, ldo=4 * Cs, out_batch_stride=(T + 2 * P) * 4 * Cs,
             flags=SPLIT | LRELU, split_off=Cs))])
         n += 2
@@ -197,7 +182,7 @@ class VocoderEngine:
                 ops.edge_pad_f16(Sin, Tin, P, 1, 2 * Ci, 2 * Ci, reflect=False)
                 n += 1
             sig = self._scaled(("convT", si), sig, calibrate, [(cv, dict(
-                A=Sin.data_ptr(), out=S.data_ptr() + 2 * (P * ld + col0), M=Tin, N=cv.N, batch=B, **self._taps(cv, [(sh, 2 * Ci, 3 * Ci, 0) for sh in shifts]),
+                A=Sin.data_ptr(), out=S.data_ptr() + 2 * (P * ld + col0), M=Tin, batch=B, spatial=[(sh, 2 * Ci, 3 * Ci, 0) for sh in shifts],
                 a_rows=Tin + 2 * P, a_cols=ldin, lda=ldin, a_batch_stride=(Tin + 2 * P) * ldin, ldo=r * ld, out_batch_stride=(T + 2 * P) * ld,
                 flags=SPLIT | DUAL, split_off=Co, dual_off=2 * Co, out_col_group=Cout, out_col_group_stride=ld))
                 for cv, shifts, col0 in ((st["ca"], (P - 1, P), 0), (st["cb"], (P, P + 1), half * ld))])
@@ -206,14 +191,14 @@ class VocoderEngine:
                 d, g1 = rb["d"], rb["g1"]
                 ops.edge_pad_f16(S, T, P, d, 2 * Co, 2 * Co, reflect=True)
                 sig_y = self._scaled(("g1", si, ri), sig, calibrate, [(g1, dict(
-                    A=S.data_ptr(), out=Y.data_ptr(), M=T, N=Cout, batch=B, **self._taps(g1, [(P + (j - 1) * d, 2 * Co, 3 * Co, 0) for j in range(3)]),
+                    A=S.data_ptr(), out=Y.data_ptr(), M=T, batch=B, spatial=[(P + (j - 1) * d, 2 * Co, 3 * Co, 0) for j in range(3)],
                     a_rows=T + 2 * P, a_cols=ld, lda=ld, a_batch_stride=(T + 2 * P) * ld, ldo=2 * Co, out_batch_stride=T * 2 * Co,
                     flags=SPLIT | LRELU, split_off=Co))])
                 if calibrate:  # x is stored at sigma, y at sigma_y: the 1x1 half of the fused weight absorbs sigma / sigma_y (a power of two)
                     rb["g2"] = _PackedConv([rb["ws"], rb["w1"] * (sig / sig_y)], rb["b2"], fold=Co == 32)
                 g2 = rb["g2"]
                 sig = self._scaled(("g2", si, ri), sig, calibrate, [(g2, dict(
-                    A=S.data_ptr(), A2=Y.data_ptr(), out=S.data_ptr() + 2 * (P * ld), M=T, N=Cout, batch=B, **self._taps(g2, [(P, 0, Co, 0), (0, 0, Co, 1)]),
+                    A=S.data_ptr(), A2=Y.data_ptr(), out=S.data_ptr() + 2 * (P * ld), M=T, batch=B, spatial=[(P, 0, Co, 0), (0, 0, Co, 1)],
                     a_rows=T + 2 * P, a_cols=ld, lda=ld, a_batch_stride=(T + 2 * P) * ld, lda2=2 * Co, a2_rows=T, a2_cols=2 * Co,
                     a2_batch_stride=T * 2 * Co, ldo=ld, out_batch_stride=(T + 2 * P) * ld, flags=SPLIT | DUAL, split_off=Co, dual_off=2 * Co,
                     # in place: ONE N tile must cover all Cout columns (a second N tile would re-read rows the first one overwrote)
@@ -228,9 +213,7 @@ class VocoderEngine:
             ops.conv_out_pair(S, T, P - 3, 2 * C, self.last_w, cv.bias, 1.0 / sig, out=wav)
             self.launches = n + 2
             return wav.view(B, 1, T)
-        tp = self._taps(cv, [(P - 3 + j, 2 * C, 3 * C, 0) for j in range(7)])
-        ops.gemm_desc(A=S.data_ptr(), W=cv.w.data_ptr(), out=wav.data_ptr(), M=T, N=1, K=64 if tp["resident_w"] else cv.Kp, batch=B, **tp,
-                      a_rows=T + 2 * P, a_cols=4 * C, lda=4 * C, a_batch_stride=(T + 2 * P) * 4 * C,
-                      ldw=cv.w.shape[1], w_cols=cv.w.shape[1], ldo=1, out_batch_stride=T, bias=cv.bias, flags=TANH, alpha=cv.alpha / sig)
+        cv.launch(A=S.data_ptr(), out=wav.data_ptr(), M=T, batch=B, spatial=[(P - 3 + j, 2 * C, 3 * C, 0) for j in range(7)], a_rows=T + 2 * P,
+                  a_cols=4 * C, lda=4 * C, a_batch_stride=(T + 2 * P) * 4 * C, ldo=1, out_batch_stride=T, bias=cv.bias, flags=TANH, alpha=1.0 / sig)
         self.launches = n + 2
         return wav.view(B, 1, T)
