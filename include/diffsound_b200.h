@@ -165,6 +165,11 @@ int dsb_silu(const float* in, float* out, long long n, void* stream);
 int dsb_attention(const float* q, long long ldq, const float* k, long long ldk, const float* v, long long ldv, float* o, long long ldo,
                   int B, int H, int Lq, int Lk, float scale, int flags, void* stream);
 
+/* dsb_attention for head_dim 32 (Diffsound caps_small_transformer.yaml: n_embd 512, 16 heads; transformer_utils.py:48-54, :99-105): the same
+ * arguments and layout, head h occupies columns [32h, 32h+32). */
+int dsb_attention_hd32(const float* q, long long ldq, const float* k, long long ldk, const float* v, long long ldv, float* o, long long ldo,
+                       int B, int H, int Lq, int Lk, float scale, int flags, void* stream);
+
 /* Same attention core with fp16 q/k/v (row strides in halves, multiples of 8); o is fp16 (DSB_GEMM_OUT_F16) or fp32.
  * flags | DSB_ATTN_CAUSAL: key j is visible to query i only if j <= i (the CLIP text transformer's mask, clip/model.py build_attention_mask). */
 #define DSB_ATTN_CAUSAL 1024
@@ -184,6 +189,11 @@ int dsb_attention_tc2(const void* q, long long ldq, const void* k, long long ldk
 int dsb_attention_tc_split(const void* q, long long ldq, long long q_lo_off, const void* k, long long ldk, long long k_lo_off, const void* v,
                            long long ldv, long long v_lo_off, void* o, long long ldo, long long o_lo_off, int B, int H, int Lq, int Lk,
                            float scale, void* stream);
+/* dsb_attention_tc_split for head_dim 32 (caps_small_transformer.yaml; transformer_utils.py:48-54, :99-105): the same arguments and pair
+ * layout, head h occupies columns [32h, 32h+32) of each half; 64-byte swizzled tiles, S = 6 and P V = 12 wgmma per 64-key chunk. */
+int dsb_attention_tc_split_hd32(const void* q, long long ldq, long long q_lo_off, const void* k, long long ldk, long long k_lo_off, const void* v,
+                                long long ldv, long long v_lo_off, void* o, long long ldo, long long o_lo_off, int B, int H, int Lq, int Lk,
+                                float scale, void* stream);
 
 
 /* ---------------------------------------------------------------------------------------------------------------

@@ -42,12 +42,14 @@ SIGNATURES = {
     "dsb_silu": [c_vp, c_vp, c_ll, c_vp],
     "dsb_split_f16": [c_vp, c_ll, c_vp, c_ll, c_ll, c_ll, c_i, c_f, c_vp],
     "dsb_attention_tc_split": [c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_i, c_i, c_i, c_i, c_f, c_vp],
+    "dsb_attention_tc_split_hd32": [c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_i, c_i, c_i, c_i, c_f, c_vp],
     "dsb_l2_normalize_rows": [c_vp, c_ll, c_i, c_vp],
     "dsb_split_tf32": [c_vp, c_ll, c_vp, c_ll, c_ll, c_i, c_i, c_i, c_vp],
     "dsb_embed_tokens": [c_vp] * 5 + [c_i] * 6 + [c_vp, c_vp],
     "dsb_layernorm": [c_vp] * 4 + [c_i, c_i, c_f, c_i, c_vp],
     "dsb_ada_layernorm": [c_vp] * 4 + [c_i] * 4 + [c_f, c_i, c_vp],
     "dsb_attention": [c_vp, c_ll, c_vp, c_ll, c_vp, c_ll, c_vp, c_ll, c_i, c_i, c_i, c_i, c_f, c_i, c_vp],
+    "dsb_attention_hd32": [c_vp, c_ll, c_vp, c_ll, c_vp, c_ll, c_vp, c_ll, c_i, c_i, c_i, c_i, c_f, c_i, c_vp],
     "dsb_codebook_gather_padded": [c_vp] * 3 + [c_i] * 6 + [c_vp, c_vp],
     "dsb_groupnorm_stats": [c_vp, c_vp] + [c_i] * 4 + [c_vp],
     "dsb_groupnorm_apply": [c_vp] * 5 + [c_i] * 5 + [c_f, c_i, c_i, c_vp],

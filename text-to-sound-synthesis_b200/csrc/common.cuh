@@ -27,10 +27,11 @@ void set_error(const char* fmt, ...);
   } while (0)
 
 int sm_count();
-// 3-D TMA map (K, rows, batch) over a K-contiguous matrix; box = (128 bytes of K, box_rows, 1); SWIZZLE_128B; OOB reads give zeros.
-// kind: DSB_DTYPE_TF32 (fp32 elements) / BF16 / F16.  Returns non-zero and sets the error string on failure.  (gemm_wgmma.cu)
+// 3-D TMA map (K, rows, batch) over a K-contiguous matrix; box = (box_bytes of K, box_rows, 1); SWIZZLE_128B for 128-byte boxes, SWIZZLE_64B
+// for 64-byte ones; OOB reads give zeros.  kind: DSB_DTYPE_TF32 (fp32 elements) / BF16 / F16.  Returns non-zero and sets the error string on
+// failure.  (gemm_wgmma.cu)
 int make_operand_map(CUtensorMap* map, const void* ptr, int kind, long long kdim, long long rows, long long batch, long long ld_elems,
-                     long long bstride_elems, int box_rows, int l2_promo_128 = 0);
+                     long long bstride_elems, int box_rows, int l2_promo_128 = 0, int box_bytes = 128);
 bool pdl_enabled();  // programmatic dependent launch (env DSB_PDL=0 disables)
 
 // Launch with the programmatic-stream-serialization attribute: the grid may be scheduled while its predecessor drains; the
@@ -170,5 +171,17 @@ __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr, uint32_t
   return d;
 }
 __device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) { return make_sw128_desc(smem_addr, 16); }
+// The same for SWIZZLE_64B (layout type 2 @62): 64-byte rows, 8-row groups 512 B apart.  K-major: advancing K by 32 bytes = +2.
+// MN-major (32 two-byte MN columns per 64-byte row, 64 K rows = 4 KB per 32 MN columns): LBO between 32-column blocks, SBO = 512 B between
+// groups of 8 K rows.  Advancing K by 16 rows = +64.
+__device__ __forceinline__ uint64_t make_sw64_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;
+  d |= static_cast<uint64_t>(512 >> 4) << 32;
+  d |= static_cast<uint64_t>(2) << 62;
+  return d;
+}
+__device__ __forceinline__ uint64_t make_sw64_kmajor_desc(uint32_t smem_addr) { return make_sw64_desc(smem_addr, 16); }
 
 }  // namespace dsb

@@ -539,19 +539,20 @@ static PFN_encodeTiled get_encode() {
 
 // 3-D map (K, rows, batch) over a K-contiguous matrix; box = (128 bytes of K, box_rows, 1); SWIZZLE_128B; OOB -> 0
 int make_operand_map(CUtensorMap* map, const void* ptr, int kind, long long kdim, long long rows, long long batch,
-                            long long ld_elems, long long bstride_elems, int box_rows, int l2_promo_128) {
+                            long long ld_elems, long long bstride_elems, int box_rows, int l2_promo_128, int box_bytes) {
   PFN_encodeTiled enc = get_encode();
   DSB_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
+  DSB_REQUIRE(box_bytes == ROW_BYTES || box_bytes == 64, "make_operand_map: box_bytes must be 128 or 64 (got %d)", box_bytes);
   const int es = kind == DSB_DTYPE_TF32 ? 4 : 2;
   DSB_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "GEMM operand pointer must be 16-byte aligned");
   DSB_REQUIRE((ld_elems * es) % 16 == 0, "GEMM operand leading dimension must be a multiple of 16 bytes (ld=%lld)", ld_elems);
   DSB_REQUIRE(batch == 1 || (bstride_elems * es) % 16 == 0, "GEMM batch stride must be a multiple of 16 bytes");
   cuuint64_t gdim[3] = {(cuuint64_t)kdim, (cuuint64_t)rows, (cuuint64_t)batch};
   cuuint64_t gstr[2] = {(cuuint64_t)(ld_elems * es), (cuuint64_t)((batch == 1 ? ld_elems * rows : bstride_elems) * es)};
-  cuuint32_t box[3] = {(cuuint32_t)(ROW_BYTES / es), (cuuint32_t)box_rows, 1};
+  cuuint32_t box[3] = {(cuuint32_t)(box_bytes / es), (cuuint32_t)box_rows, 1};
   cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = enc(map, kind == DSB_DTYPE_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : (kind == DSB_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32), 3, const_cast<void*>(ptr), gdim, gstr,
-                   box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, box_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                    // state rows [raw pair | activated pair] are read one 128-byte half at a time: a 256-byte promotion would fetch the other half too
                    l2_promo_128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   DSB_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d): k=%lld rows=%lld batch=%lld ld=%lld", (int)r, kdim, rows, batch, ld_elems);

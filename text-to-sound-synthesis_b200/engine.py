@@ -79,8 +79,11 @@ class DenoiserEngine:
         self.T = m.diffusion_step
         self.mlp_times = m.blocks[0].mlp[0].weight.shape[0] // m.n_embd
         D = self.D
-        if D % 64 or D // self.H != 64:
-            raise RuntimeError(f"kernels are specialised for head_dim 64 (n_embd={D}, n_head={self.H})")
+        if D % 64 or D % self.H or D // self.H not in (64, 32):
+            raise RuntimeError(f"kernels are specialised for head_dim 64 and 32 (n_embd={D}, n_head={self.H})")
+        self.head_dim = D // self.H
+        if self.head_dim == 32 and self.precision == "f16":
+            raise RuntimeError(f"precision 'f16' has no head_dim-32 attention (n_embd={D}, n_head={self.H}); use 'f16x3', 'tf32' or 'fp32'")
         f = lambda p: p.detach().float().contiguous()
         self.layers = []
         kv_w, kv_b = [], []
@@ -182,7 +185,8 @@ class DenoiserEngine:
             return self._forward_split(ids, kv_all, t, Lc, out)
         x2 = x.view(B * L, D)
         h2 = h.view(B * L, D)
-        scale = 1.0 / math.sqrt(64)
+        scale = 1.0 / math.sqrt(self.head_dim)
+        hd_arg = {} if self.head_dim == 64 else dict(head_dim=self.head_dim)  # the head_dim-64 calls keep their exact arguments
         n = 0
         ops.embed_tokens(ids, self.emb, self.hemb, self.wemb, out=x, err_flag=ws["err"]); n += 1
         for li, lay in enumerate(self.layers):
@@ -192,7 +196,7 @@ class DenoiserEngine:
                 # K / V staged once per head by TMA, fp16 mma.sync over 16-row slabs
                 ops.attention_tc(qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:], att, B=B, H=H, Lq=L, Lk=L, scale=scale)
             else:
-                ops.attention(qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:], att, B=B, H=H, Lq=L, Lk=L, scale=scale, round_out=rnd)
+                ops.attention(qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:], att, B=B, H=H, Lq=L, Lk=L, scale=scale, round_out=rnd, **hd_arg)
             self._linear(att, lay["wo1"], lay["bo1"], residual=x2, out=x2)
             ops.ada_layernorm(x, lay["tab2"], t, out=h, round_out=rnd)
             self._linear(h2, lay["wq2"], lay["bq2"], out=q2)
@@ -200,7 +204,7 @@ class DenoiserEngine:
             if self.precision == "f16" and Lc <= 272:
                 ops.attention_tc(q2, kv[:, :D], kv[:, D:], att, B=B, H=H, Lq=L, Lk=Lc, scale=scale)
             else:
-                ops.attention(q2, kv[:, :D], kv[:, D:], att, B=B, H=H, Lq=L, Lk=Lc, scale=scale, round_out=rnd)
+                ops.attention(q2, kv[:, :D], kv[:, D:], att, B=B, H=H, Lq=L, Lk=Lc, scale=scale, round_out=rnd, **hd_arg)
             self._linear(att, lay["wo2"], lay["bo2"], residual=x2, out=x2)
             ops.layernorm(x, lay["g2"], lay["b2"], out=h, eps=lay["eps2"], round_out=rnd)
             self._linear(h2, lay["w1"], lay["b1"], out=hid, gelu=True, round_out=rnd)
@@ -222,7 +226,8 @@ class DenoiserEngine:
         x, h, qkv, att, q2, hid = ws["x"], ws["h"], ws["qkv"], ws["att"], ws["q2"], ws["hid"]
         M = B * L
         x2, h2 = x.view(M, D), h.view(M, 2 * D)
-        scale = 1.0 / math.sqrt(64)
+        scale = 1.0 / math.sqrt(self.head_dim)
+        hd_arg = {} if self.head_dim == 64 else dict(head_dim=self.head_dim)
         kv_lo = self.n_layer * 2 * D
         n = 0
         ops.embed_tokens(ids, self.emb, self.hemb, self.wemb, out=x, err_flag=ws["err"]); n += 1
@@ -230,13 +235,13 @@ class DenoiserEngine:
             ops.ada_layernorm(x, lay["tab1"], t, out=h, split=True)
             self._linear(h2, lay["wqkv"], lay["bqkv"], out=qkv, split_out=True)
             ops.attention_tc_split(qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:3 * D], att[:, :D], q_lo=3 * D, k_lo=3 * D, v_lo=3 * D, o_lo=D,
-                                   B=B, H=H, Lq=L, Lk=L, scale=scale)
+                                   B=B, H=H, Lq=L, Lk=L, scale=scale, **hd_arg)
             self._linear(att, lay["wo1"], lay["bo1"], residual=x2, out=x2)
             ops.ada_layernorm(x, lay["tab2"], t, out=h, split=True)
             self._linear(h2, lay["wq2"], lay["bq2"], out=q2, split_out=True)
             kv = kv_all[:, li * 2 * D:]
             ops.attention_tc_split(q2[:, :D], kv[:, :D], kv[:, D:2 * D], att[:, :D], q_lo=D, k_lo=kv_lo, v_lo=kv_lo, o_lo=D,
-                                   B=B, H=H, Lq=L, Lk=Lc, scale=scale)
+                                   B=B, H=H, Lq=L, Lk=Lc, scale=scale, **hd_arg)
             self._linear(att, lay["wo2"], lay["bo2"], residual=x2, out=x2)
             ops.layernorm(x, lay["g2"], lay["b2"], out=h, eps=lay["eps2"], split=True)
             self._linear(h2, lay["w1"], lay["b1"], out=hid, gelu=True, split_out=True)

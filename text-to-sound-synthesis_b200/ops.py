@@ -328,8 +328,15 @@ def l2_normalize_rows_(x):
 ATTN_CAUSAL = 1024
 
 
-def attention(q, k, v, out, *, B, H, Lq, Lk, scale, round_out=False, causal=False):
-    """q/out: row-strided views with (B*Lq) rows; k/v: (B*Lk) rows; head h = columns [64h, 64h+64).  causal (fp16 path): key j visible to query i iff j <= i."""
+def _attention_head_dim(name, head_dim):
+    if head_dim not in (32, 64):
+        raise ValueError(f"{name}: head_dim {head_dim} unsupported (32 or 64)")
+
+
+def attention(q, k, v, out, *, B, H, Lq, Lk, scale, round_out=False, causal=False, head_dim=64):
+    """q/out: row-strided views with (B*Lq) rows; k/v: (B*Lk) rows; head h = columns [head_dim*h, head_dim*(h+1)), head_dim 64 or 32 (fp32
+    operands only at 32).  causal (fp16 path): key j visible to query i iff j <= i."""
+    _attention_head_dim("attention", head_dim)
     _need_cuda(q, k, v, out)
     for t_ in (q, k, v, out):
         if t_.stride(-1) != 1:
@@ -337,14 +344,17 @@ def attention(q, k, v, out, *, B, H, Lq, Lk, scale, round_out=False, causal=Fals
     if q.dtype == torch.float16:
         if k.dtype != torch.float16 or v.dtype != torch.float16:
             raise RuntimeError("attention: q, k, v must share a dtype")
+        if head_dim != 64:
+            raise RuntimeError(f"attention: fp16 operands need head_dim 64 (got {head_dim})")
         _lib.check(_lib.lib().dsb_attention_f16(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0), out.data_ptr(),
                                                 out.stride(0), B, H, Lq, Lk, scale, _out_flags(out, False) | (ATTN_CAUSAL if causal else 0), _stream()),
                    "dsb_attention_f16")
         return out
     if causal:
         raise RuntimeError("causal attention is implemented for fp16 operands")
-    _lib.check(_lib.lib().dsb_attention(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0), out.data_ptr(), out.stride(0),
-                                        B, H, Lq, Lk, scale, _out_flags(out, round_out), _stream()), "dsb_attention")
+    name = "dsb_attention" if head_dim == 64 else "dsb_attention_hd32"
+    _lib.check(getattr(_lib.lib(), name)(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0), out.data_ptr(), out.stride(0),
+                                         B, H, Lq, Lk, scale, _out_flags(out, round_out), _stream()), name)
     return out
 
 
@@ -362,14 +372,16 @@ def attention_tc(q, k, v, out, *, B, H, Lq, Lk, scale, pipelined=True):
     return out
 
 
-def attention_tc_split(q, k, v, out, *, q_lo, k_lo, v_lo, o_lo, B, H, Lq, Lk, scale):
-    """Split-fp16 tensor-core attention: q/k/v/out are the hi halves (row-strided fp16 views, head h = columns [64h, 64h+64)); the matching lo half
-    of every row lies *_lo elements further along the row."""
+def attention_tc_split(q, k, v, out, *, q_lo, k_lo, v_lo, o_lo, B, H, Lq, Lk, scale, head_dim=64):
+    """Split-fp16 tensor-core attention: q/k/v/out are the hi halves (row-strided fp16 views, head h = columns [head_dim*h, head_dim*(h+1)),
+    head_dim 64 or 32); the matching lo half of every row lies *_lo elements further along the row."""
+    _attention_head_dim("attention_tc_split", head_dim)
     _need_cuda(q, k, v, out)
     if not all(t_.dtype == torch.float16 and t_.stride(-1) == 1 for t_ in (q, k, v, out)):
         raise RuntimeError("attention_tc_split needs fp16 tensors contiguous in the head dimension")
-    _lib.check(_lib.lib().dsb_attention_tc_split(q.data_ptr(), q.stride(0), q_lo, k.data_ptr(), k.stride(0), k_lo, v.data_ptr(), v.stride(0), v_lo,
-                                                 out.data_ptr(), out.stride(0), o_lo, B, H, Lq, Lk, scale, _stream()), "dsb_attention_tc_split")
+    name = "dsb_attention_tc_split" if head_dim == 64 else "dsb_attention_tc_split_hd32"
+    _lib.check(getattr(_lib.lib(), name)(q.data_ptr(), q.stride(0), q_lo, k.data_ptr(), k.stride(0), k_lo, v.data_ptr(), v.stride(0), v_lo,
+                                         out.data_ptr(), out.stride(0), o_lo, B, H, Lq, Lk, scale, _stream()), name)
     return out
 
 

@@ -52,6 +52,12 @@ def build_diffusion_transformer(K, D, NL, NH, CD, sd=None, spatial=(5, 53), T=10
     return m.cuda().eval()
 
 
+# Diffsound/configs/ denoisers by (num_embed, n_embd, n_layer, n_head): caps_small_transformer.yaml differs from caps.yaml in n_layer, n_embd and
+# the position embed_dim (= n_embd here), so its heads are 32 wide; build_dalle(**DALLE_CONFIGS[name]) builds one
+DALLE_CONFIGS = {"caps": dict(K=256, D=1024, NL=19, NH=16), "caps_2048": dict(K=2048, D=1024, NL=19, NH=16),
+                 "caps_small_transformer": dict(K=256, D=512, NL=18, NH=16)}
+
+
 def build_dalle(K=256, D=1024, NL=19, NH=16, CD=512, precision=None, seed=0):
     """The full caps.yaml model (DALLE = SpecVQGAN codec + ColumnMajor + DiffusionTransformer), seeded random init, on the GPU."""
     torch.manual_seed(seed)
