@@ -377,6 +377,26 @@ int dsb_pair_channel_mean(const void* in, long long ld, long long lo_off, int Hp
                           float* out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
+ * SpecVQGAN log-mel spectrogram (reference Codebook/feature_extraction/extract_mel_spectrogram.py: MelSpectrogram :15-38, the transforms
+ * :40-139, TRANSFORMS :141-151, get_spectrogram :166-187; librosa 0.8.0: stft(n_fft 1024, hop 256, center, reflect, periodic Hann),
+ * filters.mel(22050, 1024, fmin 125, fmax 7600, 80 mels, Slaney) in float32).  The DFT between the two entry points is a dsb_gemm_ex
+ * split-fp16 4-tap conv over the frames buffer: frame t = rows t ... t+3, K = 256 per tap, W = windowed cos / -sin pairs of the bins that
+ * any filter covers, fp32 out.
+ * ------------------------------------------------------------------------------------------------------------- */
+#define DSB_WAV_SCALE 8192.0f /* 2^13: samples are stored scaled so that lo halves stay in fp16's normal range; the GEMM alpha undoes it */
+#define DSB_WAV_LIMIT 4.0f    /* |x| must be below this (x * 2^13 < 2^15 stays finite in fp16) */
+/* wav (B, length) fp32, row stride ld_wav -> out (B, rows, 512) fp16: row r holds padded samples [256 r, 256 r + 256) of the clip
+ * reflect-padded by 512 on each side (numpy.pad mode='reflect', librosa.stft center=True), as hi = f16(2^13 x) at [0, 256) and
+ * lo = f16(2^13 x - hi) at [256, 512); samples past the padded end are zero.  rows >= length / 256 + 4 (frames 1 + length / 256 need rows up to
+ * length / 256 + 3).  length > 512.  A sample that is not finite or has |x| >= DSB_WAV_LIMIT sets *err_flag (may be NULL). */
+int dsb_wav_frames_f16(const float* wav, long long ld_wav, int B, int length, void* out_f16, int rows, int* err_flag, void* stream);
+/* spec (B, T, ld_spec) fp32, bin k of frame t at columns (2k, 2k + 1) = (re, im) -> out (B, n_mels, T_out) fp32, T_out <= T:
+ * mel[m, t] = sum_{i < fb_len[m]} fb_w[m * fb_ld + i] * |X[t, fb_start[m] + i]| (fp32, ascending i; |X| = sqrt(re^2 + im^2) in fp32), then
+ * max(., 1e-5), log10, * 20, - 20, + 100, / 100, clip(0, 1), each step rounded in fp32 in the reference's order.  n_bins <= 383. */
+int dsb_mel_log(const float* spec, long long ld_spec, long long spec_batch_stride, int B, int T, int T_out, int n_bins, const int* fb_start,
+                const int* fb_len, const float* fb_w, int fb_ld, int n_mels, float* out, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
  * Training (SURVEY.md section 8 row A13; reference sound_synthesis/modeling/transformers/diffusion_transformer.py:370-377, :408-476).
  * The reference obtains every gradient below from torch autograd; these entry points are the hand-written backward passes.
  * "dtype" selects the activation storage: DSB_DTYPE_TF32 (fp32 containers, tf32-rounded on store) or DSB_DTYPE_BF16.

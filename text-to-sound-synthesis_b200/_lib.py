@@ -82,6 +82,9 @@ SIGNATURES = {
     "dsb_pair_maxpool3s2": [c_vp] + [c_i] * 6 + [c_vp, c_ll, c_ll] + [c_i] * 6 + [c_f, c_vp],
     "dsb_pair_avgpool3": [c_vp] + [c_i] * 6 + [c_vp, c_ll, c_ll, c_i, c_i, c_vp],
     "dsb_pair_channel_mean": [c_vp, c_ll, c_ll] + [c_i] * 8 + [c_f, c_vp, c_vp],
+    # SpecVQGAN log-mel spectrogram
+    "dsb_wav_frames_f16": [c_vp, c_ll, c_i, c_i, c_vp, c_i, c_vp, c_vp],
+    "dsb_mel_log": [c_vp, c_ll, c_ll] + [c_i] * 4 + [c_vp] * 3 + [c_i, c_i, c_vp, c_vp],
     # training (A13)
     "dsb_q_sample": [c_vp] * 5 + [c_i] * 4 + [c_vp],
     "dsb_train_loss": [c_vp] * 16 + [c_i] * 4 + [c_f, c_i, c_f, c_f, c_i, c_vp],

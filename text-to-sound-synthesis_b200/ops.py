@@ -679,3 +679,42 @@ def check_ar_sampler_args(V, top_k, temperature):
         raise ValueError(f"top_k={top_k} out of range: torch.topk needs 1 <= k <= vocab size ({V})")
     if not float(temperature) == float(temperature) or float(temperature) == 0.0:
         raise ValueError("temperature must be a non-zero number")
+
+
+# ---------------------------------------------------------------- SpecVQGAN log-mel spectrogram (mel.cu)
+WAV_SCALE = 8192.0  # DSB_WAV_SCALE
+WAV_LIMIT = 4.0     # DSB_WAV_LIMIT
+MEL_HOP, MEL_PAD = 256, 512
+
+
+def wav_frame_rows(length: int) -> int:
+    """Rows per clip dsb_wav_frames_f16 needs: frames 1 + length // 256, frame t = rows t ... t+3."""
+    return length // MEL_HOP + 4
+
+
+def wav_frames_f16(wav, out=None, *, rows=None, err_flag=None):
+    """wav (B, length) fp32, contiguous in time -> (B, rows, 512) fp16: the reflect-padded clip as rows of 256 samples, [hi | lo] of 2^13 x."""
+    _need_cuda(wav, out, err_flag)
+    if wav.dim() != 2 or wav.dtype != torch.float32 or wav.stride(1) != 1:
+        raise RuntimeError("wav_frames_f16 needs a (B, length) fp32 tensor contiguous in time")
+    B, length = wav.shape
+    rows = wav_frame_rows(length) if rows is None else rows
+    if out is None:
+        out = torch.empty(B, rows, 2 * MEL_HOP, dtype=torch.float16, device=wav.device)
+    _lib.check(_lib.lib().dsb_wav_frames_f16(wav.data_ptr(), wav.stride(0), B, length, out.data_ptr(), rows, _ptr(err_flag), _stream()),
+               "dsb_wav_frames_f16")
+    return out
+
+
+def mel_log(spec, n_bins, fb_start, fb_len, fb_w, T_out, out=None):
+    """spec (B, T, ld) fp32 interleaved (re, im) pairs of n_bins DFT bins -> (B, n_mels, T_out) SpecVQGAN log-mel (see dsb_mel_log)."""
+    _need_cuda(spec, fb_start, fb_len, fb_w, out)
+    B, T, ld = spec.shape
+    n_mels, fb_ld = fb_w.shape
+    if spec.stride(2) != 1 or spec.stride(1) != ld:
+        raise RuntimeError("mel_log needs (B, T, ld) spectra with contiguous rows")
+    if out is None:
+        out = torch.empty(B, n_mels, T_out, dtype=torch.float32, device=spec.device)
+    _lib.check(_lib.lib().dsb_mel_log(spec.data_ptr(), ld, spec.stride(0), B, T, T_out, n_bins, fb_start.data_ptr(), fb_len.data_ptr(), fb_w.data_ptr(),
+                                      fb_ld, n_mels, out.data_ptr(), _stream()), "dsb_mel_log")
+    return out
