@@ -194,6 +194,13 @@ int dsb_attention_tc_split(const void* q, long long ldq, long long q_lo_off, con
 int dsb_attention_tc_split_hd32(const void* q, long long ldq, long long q_lo_off, const void* k, long long ldk, long long k_lo_off, const void* v,
                                 long long ldv, long long v_lo_off, void* o, long long ldo, long long o_lo_off, int B, int H, int Lq, int Lk,
                                 float scale, void* stream);
+/* Causal dsb_attention_tc_split (Codebook/specvqgan/modules/transformer/mingpt.py:76-94 CausalSelfAttention, n_unmasked = 0:
+ *   att = att.masked_fill(self.mask[:,:,:T,:T] == 0, float('-inf'))  -- key j of query row i is dropped when j > i, condition rows included)
+ * for head_dim 64 or 32 (the arguments of dsb_attention_tc_split / _hd32 plus head_dim).  Lq must equal Lk.  A 64-row query tile t multiplies the
+ * 64-key chunks 0 ... t only; chunks past the diagonal are neither loaded nor multiplied. */
+int dsb_attention_tc_split_causal(const void* q, long long ldq, long long q_lo_off, const void* k, long long ldk, long long k_lo_off, const void* v,
+                                  long long ldv, long long v_lo_off, void* o, long long ldo, long long o_lo_off, int B, int H, int Lq, int Lk,
+                                  float scale, int head_dim, void* stream);
 
 
 /* ---------------------------------------------------------------------------------------------------------------
@@ -277,6 +284,21 @@ int dsb_ar_embed(const float* cond, const float* tok_emb, const float* pos_emb, 
  * reads nothing. */
 int dsb_ar_attention(const float* qkv, long long ld_qkv, float* k_cache, float* v_cache, long long cache_ld, int max_pos, void* out, long long ld_out,
                      long long lo_off, const unsigned long long* ctrl, int B, int H, int head_dim, float scale, void* stream);
+/* The full-sequence forward (scoring) of the same model, every position at once (mingpt.py:161-169):
+ *   token_embeddings = self.tok_emb(idx); token_embeddings = torch.cat((embeddings, token_embeddings), dim=1)
+ *   x = self.drop(token_embeddings + position_embeddings)
+ * x[b, t, :] = (t < Tc ? cond[b, t, :] : tok_emb[ids[b * ids_ld + t - Tc], :]) + pos_emb[t, :] for t < T, x (B, T, D) fp32, the fp32 sum of
+ * dsb_ar_embed.  An id outside [0, V) sets *err_flag and reads row 0. */
+int dsb_ar_embed_all(const float* cond, const float* tok_emb, const float* pos_emb, const int64_t* ids, long long ids_ld, float* x, int B, int T,
+                     int Tc, int V, int D, int* err_flag, void* stream);
+/* GPT.forward's loss (mingpt.py:183-185) and Net2NetTransformer.shared_step's (cond_transformer.py:106, :358-359):
+ *   logits = logits[:, cond_size-1:];  loss = F.cross_entropy(logits.reshape(-1, logits.size(-1)), target.reshape(-1))
+ * logits fp32 (B, T, V), row (b, t) at logits + (b * T + t) * ld; the window is rows r0 ... r0 + n - 1 of every batch item; targets int64 (B, n)
+ * (row stride tgt_ld).  nll (B, n): the per-row -log_softmax at the target (0 at ignore_index -100), each row reduced by one CTA in a fixed
+ * order (independent of B); loss (1): the mean of the non-ignored rows, summed in fp64 in ascending row order (NaN when every row is ignored).
+ * A target outside [0, V) other than -100 sets *err_flag (its nll is NaN).  V <= 4096. */
+int dsb_ar_cross_entropy(const float* logits, long long ld, int T, int r0, int n, const int64_t* targets, long long tgt_ld, float* nll, float* loss,
+                         int B, int V, int* err_flag, void* stream);
 /* nn.GELU() (exact erf form, mingpt.py:104-109) between the MLP GEMMs: y = x * 0.5 * (1 + erff(x / sqrt(2))) of fp32 in (rows, C), written
  * as the fp16 (hi | lo) pair (hi at out[r * ld_out + c], lo lo_off halves further). */
 int dsb_gelu_erf_split(const float* in, long long ld_in, void* out, long long ld_out, long long lo_off, int rows, int C, void* stream);

@@ -43,6 +43,7 @@ SIGNATURES = {
     "dsb_split_f16": [c_vp, c_ll, c_vp, c_ll, c_ll, c_ll, c_i, c_f, c_vp],
     "dsb_attention_tc_split": [c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_i, c_i, c_i, c_i, c_f, c_vp],
     "dsb_attention_tc_split_hd32": [c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_i, c_i, c_i, c_i, c_f, c_vp],
+    "dsb_attention_tc_split_causal": [c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_vp, c_ll, c_ll, c_i, c_i, c_i, c_i, c_f, c_i, c_vp],
     "dsb_l2_normalize_rows": [c_vp, c_ll, c_i, c_vp],
     "dsb_split_tf32": [c_vp, c_ll, c_vp, c_ll, c_ll, c_i, c_i, c_i, c_vp],
     "dsb_embed_tokens": [c_vp] * 5 + [c_i] * 6 + [c_vp, c_vp],
@@ -74,6 +75,8 @@ SIGNATURES = {
     # autoregressive transformer decode
     "dsb_ar_embed": [c_vp] * 4 + [c_ll, c_vp, c_vp] + [c_i] * 4 + [c_vp, c_vp],
     "dsb_ar_attention": [c_vp, c_ll, c_vp, c_vp, c_ll, c_i, c_vp, c_ll, c_ll, c_vp, c_i, c_i, c_i, c_f, c_vp],
+    "dsb_ar_embed_all": [c_vp] * 4 + [c_ll, c_vp] + [c_i] * 5 + [c_vp, c_vp],
+    "dsb_ar_cross_entropy": [c_vp, c_ll, c_i, c_i, c_i, c_vp, c_ll, c_vp, c_vp, c_i, c_i, c_vp, c_vp],
     "dsb_gelu_erf_split": [c_vp, c_ll, c_vp, c_ll, c_ll, c_i, c_i, c_vp],
     "dsb_ar_sample": [c_vp, c_ll, c_vp, c_ll, c_vp, c_i, c_i, c_i, c_f, c_i, c_i, c_vp, c_vp, c_ll, c_vp, c_vp],
     # Melception feature extractor

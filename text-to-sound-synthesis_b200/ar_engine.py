@@ -10,6 +10,12 @@ arithmetic.  One position of B rows is a fixed launch sequence (dsb_ar_* in incl
 The current position and the RNG state live in a device loop-control block that the sampler's last CTA advances, so the step is captured once as
 a CUDA graph and replayed for every position.  Teacher-forced forward() runs the same steps and records every position's logits.  One precision:
 every GEMM operand is an fp16 (hi | lo) pair ('f16x3', fp32-class results); the attention, softmax and sampler arithmetic is fp32.
+
+Scoring (GPT.forward with targets, Net2NetTransformer.shared_step) knows the whole sequence up front, so prefill() runs every position in one pass
+with M = B * T GEMMs on the same packed weights and one CUDA graph, for the latest (B, T):
+
+    embed all, n_layer x [LayerNorm, QKV (split pair out), causal split attention, proj + residual, LayerNorm, MLP1, GELU(erf) + split,
+    MLP2 + residual], ln_f, head, cross-entropy
 """
 from __future__ import annotations
 
@@ -29,6 +35,7 @@ class AREngine:
         self.use_cuda_graph = use_cuda_graph
         self.packed = False
         self._ws: Dict[int, dict] = {}
+        self._pf: Dict[tuple, dict] = {}  # the prefill workspace of the latest (B, T)
         self.generation = 0  # bumped by repack(): graphs that baked old pointers are rebuilt
         self._param_sig = None
         self.launches_per_step = 0
@@ -82,6 +89,7 @@ class AREngine:
         self.packed = True
         self.generation += 1
         self._ws.clear()
+        self._pf.clear()
 
     # ------------------------------------------------------------------ workspaces
     def workspace(self, B: int) -> dict:
@@ -203,6 +211,94 @@ class AREngine:
         out_ids = ws["ids"][:, :n_pos - Tc + 1].clone() if first < n_pos else None
         out_hist = hist[:, :n_pos].clone() if record_logits else None
         return out_ids, out_hist
+
+    # ------------------------------------------------------------------ full-sequence forward (scoring)
+    def prefill_workspace(self, B: int, T: int) -> dict:
+        """Buffers of prefill() for one (B, T): the (B * T)-row activations, logits, the static inputs of the captured graph and its graphs.  About
+        B * T * (60 D + 4 V) bytes (1.06 GB at caps_transformer width, B = 64, T = 265), so only the latest shape is kept: a new (B, T) frees the old
+        workspace and its graphs first."""
+        ws = self._pf.get((B, T))
+        if ws is None:
+            self._pf.clear()
+            dev, D, V, M = self.device, self.D, self.V, B * T
+            e = lambda *s: torch.empty(*s, dtype=torch.float32, device=dev)
+            pair = lambda r, c: torch.zeros(r, 2 * c, dtype=torch.float16, device=dev)
+            ws = dict(x=e(B, T, D), h=pair(M, D), qkv=pair(M, 3 * D), att=pair(M, D), hid=e(M, 4 * D), hid2=pair(M, 4 * D), logits=e(B, T, V),
+                      cond=torch.zeros(B * T * D, dtype=torch.float32, device=dev), ids=torch.zeros(B, T, dtype=torch.int64, device=dev),
+                      tgt=torch.zeros(B, T, dtype=torch.int64, device=dev), nll=e(B * T), loss=e(()),
+                      err=torch.zeros(2, dtype=torch.int32, device=dev), graphs={})
+            self._pf[(B, T)] = ws
+        return ws
+
+    def _prefill_step(self, ws, B: int, T: int, Tc: int, first_row: int, n: int) -> None:
+        """The full-sequence launch sequence (no host reads, capturable); n = 0: no cross-entropy."""
+        D, H, V, M = self.D, self.H, self.V, B * T
+        x2, h, qkv, att, hid, hid2 = ws["x"].view(M, D), ws["h"], ws["qkv"], ws["att"], ws["hid"], ws["hid2"]
+        scale = 1.0 / math.sqrt(D // H)
+        cond = ws["cond"][:B * Tc * D].view(B, Tc, D)
+        ops.ar_embed_all(cond, self.tok_emb, self.pos_emb, ws["ids"][:, :T - Tc], ws["x"], err_flag=ws["err"][0:1])
+        for lay in self.layers:
+            ops.layernorm(x2, lay["g1"], lay["b1"], out=h, eps=lay["eps1"], split=True)
+            ops.gemm_f16x3(h, lay["wqkv"].pair, lay["bqkv"], out=qkv, alpha=lay["wqkv"].alpha, split_out=True)  # [Qh Kh Vh | Ql Kl Vl]
+            ops.attention_tc_split_causal(qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:3 * D], att[:, :D], q_lo=3 * D, k_lo=3 * D, v_lo=3 * D, o_lo=D,
+                                          B=B, H=H, L=T, scale=scale, head_dim=D // H)
+            ops.gemm_f16x3(att, lay["wo"].pair, lay["bo"], residual=x2, out=x2, alpha=lay["wo"].alpha)
+            ops.layernorm(x2, lay["g2"], lay["b2"], out=h, eps=lay["eps2"], split=True)
+            ops.gemm_f16x3(h, lay["w1"].pair, lay["bm1"], out=hid, alpha=lay["w1"].alpha)
+            ops.gelu_erf_split(hid, out=hid2)
+            ops.gemm_f16x3(hid2, lay["w2"].pair, lay["bm2"], residual=x2, out=x2, alpha=lay["w2"].alpha)
+        ops.layernorm(x2, self.gf, self.bf, out=h, eps=self.epsf, split=True)
+        ops.gemm_f16x3(h, self.whead.pair, None, out=ws["logits"].view(M, V), alpha=self.whead.alpha)
+        if n:
+            ops.ar_cross_entropy(ws["logits"], ws["tgt"][:, :n], first_row=first_row, nll=ws["nll"][:B * n].view(B, n), loss=ws["loss"],
+                                 err_flag=ws["err"][1:2])
+
+    @torch.no_grad()
+    def prefill(self, cond: torch.Tensor, ids: torch.Tensor, targets: Optional[torch.Tensor] = None, first_row: int = 0):
+        """Every position's logits in one causal pass: cond (B, Tc, D) fp32 (the embedded condition), ids (B, T - Tc) tokens.  With targets
+        (B, n) int64 (ignore_index -100), also F.cross_entropy over logits rows first_row ... first_row + n - 1.  Returns (logits (B, T, V),
+        loss () or None, per-row NLL (B, n) or None)."""
+        self.ensure_current()
+        B, Tc, _ = cond.shape
+        T = Tc + ids.shape[1]
+        n = 0 if targets is None else targets.shape[1]
+        if targets is not None and (targets.shape[0] != B or not 0 <= first_row <= T - n):
+            raise ValueError(f"targets {tuple(targets.shape)} do not fit rows {first_row} ... of {B} x {T} logits")
+        ws = self.prefill_workspace(B, T)
+        if Tc:
+            ws["cond"][:B * Tc * self.D].view(B, Tc, self.D).copy_(cond)
+        ws["ids"][:, :T - Tc].copy_(ids)
+        if n:
+            ws["tgt"][:, :n].copy_(targets)
+        key = (Tc, first_row, n)
+        g = ws["graphs"].get(key) if self.use_cuda_graph else None
+        if g is not None and g[1] != self.generation:
+            g = None
+        if self.use_cuda_graph and g is None:
+            dev = self.device
+            s = torch.cuda.Stream(device=dev)  # warm-up on a side stream (lazy inits), then capture
+            s.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(s):
+                self._prefill_step(ws, B, T, Tc, first_row, n)
+            torch.cuda.current_stream(dev).wait_stream(s)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                self._prefill_step(ws, B, T, Tc, first_row, n)
+            g = (graph, self.generation)
+            ws["graphs"][key] = g
+        if g is not None:
+            g[0].replay()
+        else:
+            self._prefill_step(ws, B, T, Tc, first_row, n)
+        err = ws["err"].tolist()  # one 8-byte read per call
+        if any(err):
+            ws["err"].zero_()
+            if err[0]:
+                raise IndexError(f"index out of range in self: a token id >= vocab_size ({self.V}) reached GPT.tok_emb")
+            raise IndexError(f"Target out of bounds: a target outside [0, {self.V}) that is not ignore_index (-100)")
+        if not n:
+            return ws["logits"].clone(), None, None
+        return ws["logits"].clone(), ws["loss"].clone(), ws["nll"][:B * n].view(B, n).clone()
 
 
 def check_ar_shapes(V: int, D: int, H: int, block_size: int) -> None:

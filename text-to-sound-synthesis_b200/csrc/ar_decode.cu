@@ -8,6 +8,8 @@
 //   [0] seed  [1] philox offset  [2] offset increment per sampled position  [3] ATen's thread count (256 * grid)  [4] position p
 //   [5] number of positions  [6] first position that samples  [7] CTA ticket
 // A position at or past [5] is a no-op in every kernel (a replay past the end writes nothing).
+// The full-sequence forward (scoring: Net2NetTransformer.shared_step) uses dsb_ar_embed_all for every position at once and dsb_ar_cross_entropy
+// on the head's logits; its attention is dsb_attention_tc_split_causal.
 #include "common.cuh"
 #include "diffsound_b200.h"
 #include "philox.cuh"
@@ -69,6 +71,86 @@ __global__ void ar_embed_kernel(const float* __restrict__ cond, const float* __r
   }
   const float* pe = pos_emb + p * D;
   for (int d = threadIdx.x; d < D; d += blockDim.x) x[(long long)b * D + d] = src[d] + pe[d];
+}
+
+// ---- embed of every position: x[b, t] = (t < Tc ? cond[b, t] : tok_emb[ids[b, t - Tc]]) + pos_emb[t], t < T  (the same fp32 sum as ar_embed)
+__global__ void ar_embed_all_kernel(const float* __restrict__ cond, const float* __restrict__ tok_emb, const float* __restrict__ pos_emb,
+                                    const int64_t* __restrict__ ids, long long ids_ld, float* __restrict__ x, int T, int Tc, int V, int D, int* err) {
+  const int t = blockIdx.x, b = blockIdx.y;
+  const float* src;
+  if (t < Tc) {
+    src = cond + ((long long)b * Tc + t) * D;
+  } else {
+    long long id = ids[(long long)b * ids_ld + (t - Tc)];
+    if (id < 0 || id >= V) {
+      if (threadIdx.x == 0 && err) atomicExch(err, 1);
+      id = 0;
+    }
+    src = tok_emb + id * D;
+  }
+  const float* pe = pos_emb + (long long)t * D;
+  float* xr = x + ((long long)b * T + t) * D;
+  for (int d = threadIdx.x; d < D; d += blockDim.x) xr[d] = src[d] + pe[d];
+}
+
+// ---- cross-entropy of one logits row per CTA (F.cross_entropy, reduction 'none', ignore_index -100), rows r0 ... r0 + n - 1 of every batch item:
+//   m = max_k l_k;  S = sum_k expf(l_k - m) (thread-strided ascending k, then cta_reduce);  nll = logf(S) - (l_y - m);  an ignored row is 0.
+// A target outside [0, V) (other than -100) sets err and writes NaN.  Nothing depends on B.
+__global__ void __launch_bounds__(ANT) ar_xent_rows_kernel(const float* __restrict__ logits, long long ld, int T, int r0, int n,
+                                                           const int64_t* __restrict__ targets, long long tgt_ld, float* __restrict__ nll, int V, int* err) {
+  __shared__ float red[ANW];
+  const int i = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+  const long long y = targets[(long long)b * tgt_ld + i];
+  float* out = nll + (long long)b * n + i;
+  if (y == -100) {
+    if (tid == 0) *out = 0.f;
+    return;
+  }
+  if (y < 0 || y >= V) {
+    if (tid == 0) {
+      *out = NAN;
+      if (err) atomicExch(err, 1);
+    }
+    return;
+  }
+  const float* row = logits + ((long long)b * T + r0 + i) * ld;
+  float mx = -INFINITY;
+  for (int k = tid; k < V; k += ANT) mx = fmaxf(mx, row[k]);
+  mx = cta_reduce(mx, red, [](float a, float c) { return fmaxf(a, c); });
+  float se = 0.f;
+  for (int k = tid; k < V; k += ANT) se += expf(row[k] - mx);
+  se = cta_reduce(se, red, [](float a, float c) { return a + c; });
+  if (tid == 0) *out = logf(se) - (row[y] - mx);
+}
+
+// ---- mean over the non-ignored rows: the fp64 NLLs added by one thread in ascending row order (b-major), staged through shared memory in chunks
+// (an ignored row enters as +0.0, which leaves every partial sum unchanged); the count is an integer sum.  0 rows give 0 / 0 = NaN, as
+// F.cross_entropy does.
+constexpr int XENT_CHUNK = 2048;
+__global__ void __launch_bounds__(ANT) ar_xent_mean_kernel(const float* __restrict__ nll, const int64_t* __restrict__ targets, long long tgt_ld, int B,
+                                                           int n, float* loss) {
+  __shared__ double vals[XENT_CHUNK];
+  __shared__ int redi[ANW];
+  const long long rows = (long long)B * n;
+  double sum = 0.0;
+  int cnt = 0;
+  for (long long c0 = 0; c0 < rows; c0 += XENT_CHUNK) {
+    const int len = (int)min((long long)XENT_CHUNK, rows - c0);
+    for (int i = threadIdx.x; i < len; i += ANT) {
+      const long long r = c0 + i, b = r / n;
+      const bool keep = targets[b * tgt_ld + (r - b * n)] != -100;
+      vals[i] = keep ? (double)nll[r] : 0.0;
+      cnt += keep ? 1 : 0;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+#pragma unroll 8
+      for (int i = 0; i < len; ++i) sum += vals[i];
+    }
+    __syncthreads();
+  }
+  cnt = cta_reduce(cnt, redi, [](int a, int e) { return a + e; });
+  if (threadIdx.x == 0) *loss = (float)(sum / (double)cnt);
 }
 
 // ---- decode attention for one (head, b) at position p  (mingpt.py:76-94 with a KV cache)
@@ -288,6 +370,29 @@ extern "C" int dsb_ar_embed(const float* cond, const float* tok_emb, const float
   DSB_REQUIRE(B > 0 && Tc >= 0 && V > 0 && D > 0, "dsb_ar_embed: bad shape");
   DSB_REQUIRE((cond || Tc == 0) && tok_emb && pos_emb && ids && x && ctrl, "dsb_ar_embed: null argument");  // no condition rows: cond unused
   ar_embed_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(cond, tok_emb, pos_emb, ids, ids_ld, x, ctrl, Tc, V, D, err_flag);
+  DSB_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dsb_ar_embed_all(const float* cond, const float* tok_emb, const float* pos_emb, const int64_t* ids, long long ids_ld, float* x, int B,
+                                int T, int Tc, int V, int D, int* err_flag, void* stream) {
+  DSB_REQUIRE(B > 0 && B <= 65535 && T > 0 && Tc >= 0 && Tc <= T && V > 0 && D > 0, "dsb_ar_embed_all: bad shape (B=%d T=%d Tc=%d)", B, T, Tc);
+  DSB_REQUIRE((cond || Tc == 0) && tok_emb && pos_emb && (ids || Tc == T) && x, "dsb_ar_embed_all: null argument");
+  ar_embed_all_kernel<<<dim3(T, B), 256, 0, (cudaStream_t)stream>>>(cond, tok_emb, pos_emb, ids, ids_ld, x, T, Tc, V, D, err_flag);
+  DSB_CHECK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int dsb_ar_cross_entropy(const float* logits, long long ld, int T, int r0, int n, const int64_t* targets, long long tgt_ld, float* nll,
+                                    float* loss, int B, int V, int* err_flag, void* stream) {
+  DSB_REQUIRE(B > 0 && B <= 65535 && n > 0 && r0 >= 0 && r0 + n <= T && V > 0 && ld >= V, "dsb_ar_cross_entropy: bad shape (B=%d T=%d r0=%d n=%d V=%d)",
+              B, T, r0, n, V);
+  DSB_REQUIRE(V <= ANT * AR_MAX_CAP, "dsb_ar_cross_entropy: V=%d too large (max %d)", V, ANT * AR_MAX_CAP);
+  DSB_REQUIRE(logits && targets && nll && loss, "dsb_ar_cross_entropy: null argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  ar_xent_rows_kernel<<<dim3(n, B), ANT, 0, st>>>(logits, ld, T, r0, n, targets, tgt_ld, nll, V, err_flag);
+  DSB_CHECK_CUDA(cudaGetLastError());
+  ar_xent_mean_kernel<<<1, ANT, 0, st>>>(nll, targets, tgt_ld, B, n, loss);
   DSB_CHECK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -13,7 +13,8 @@
 //
 // A head row is HD fp16 = 2 * HD bytes, and that is the swizzle width of every tile: SWIZZLE_128B at head_dim 64, SWIZZLE_64B at 32 (TMA
 // boxes of HD columns x 64 rows, wgmma descriptors of the same layout).  Each instantiation lives in its own translation unit:
-// attention_tc_split.cu (64) and attention_tc_split_hd32.cu (32).
+// attention_tc_split.cu (64) and attention_tc_split_hd32.cu (32); attention_tc_split_causal.cu holds both with CAUSAL set (the autoregressive
+// transformer's masked self-attention, Lq == Lk).
 #pragma once
 #include "common.cuh"
 #include "diffsound_b200.h"
@@ -80,7 +81,8 @@ __device__ __forceinline__ void at_pv(float (&part)[HD / 2], const uint32_t (&a)
 
 // One consumer warpgroup, one 64-row query tile (Q hi / lo staged at sq) against every K / V chunk of its (batch, head).
 // Accumulator fragment: this thread's rows are wq*16 + lane/4 (r0) and + 8 (r1); entry 4j + {0,1} / {2,3} is column 8j + 2(lane%4) + {0,1}.
-template <int HD>
+// CAUSAL (Lq == Lk): the tile multiplies chunks 0 ... tile only and masks key > row on the diagonal chunk.
+template <int HD, bool CAUSAL>
 __device__ __forceinline__ void at_tile(const AtParams& p, uint8_t* ring, uint64_t* full, uint64_t* empty, int& stage, uint32_t& phase, uint8_t* sq,
                                         int b, int h, int tile, int wg, int wq, int lane) {
   using C = AtCfg<HD>;
@@ -90,7 +92,7 @@ __device__ __forceinline__ void at_tile(const AtParams& p, uint8_t* ring, uint64
 #pragma unroll
   for (int i = 0; i < C::ACC; ++i) o[i] = 0.f;
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-  for (int c = 0; c < p.n_chunks; ++c) {
+  for (int c = 0; c < (CAUSAL ? tile + 1 : p.n_chunks); ++c) {
     mbar_wait(&full[stage], phase);
     const uint32_t sk = smem_u32(ring + stage * C::STAGE_BYTES);
     wgmma_fence_regs(s);
@@ -107,7 +109,20 @@ __device__ __forceinline__ void at_tile(const AtParams& p, uint8_t* ring, uint64
     wgmma_wait<0>();
     wgmma_fence_regs(s);
 
-    if ((c + 1) * 64 > p.Lk) {  // keys past Lk (zero rows from the TMA bounds) never enter the softmax
+    if constexpr (CAUSAL) {
+      // only the diagonal chunk (c == tile) holds keys past a row; they include every key past Lk of a stored row (row < Lq = Lk)
+      if (c == tile) {
+        const int r0 = wq * 16 + (lane >> 2), r1 = r0 + 8;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int key = j * 8 + 2 * t;
+          if (key > r0) s[4 * j] = -INFINITY;
+          if (key + 1 > r0) s[4 * j + 1] = -INFINITY;
+          if (key > r1) s[4 * j + 2] = -INFINITY;
+          if (key + 1 > r1) s[4 * j + 3] = -INFINITY;
+        }
+      }
+    } else if ((c + 1) * 64 > p.Lk) {  // keys past Lk (zero rows from the TMA bounds) never enter the softmax
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const int key = c * 64 + j * 8 + 2 * t;
@@ -196,7 +211,16 @@ __device__ __forceinline__ void at_tile(const AtParams& p, uint8_t* ring, uint64
   fence_proxy_async_smem();  // these generic reads / writes come before the TMA that refills the tile
 }
 
-template <int HD>
+// Unit u -> (batch, head, tile pair).  Non-causal units run head-major: u = bh * n_pairs + pair.  Causal units run heaviest pair first,
+// u = (n_pairs - 1 - pair) * (B * H) + bh, so the persistent CTAs start on the longest key streams and end on the shortest (DESIGN.md
+// section 4g); a causal unit streams the K / V chunks up to the diagonal of its pair's odd tile.  Written as constexpr-selected initialisers
+// rather than a helper so that the non-causal instantiations compile to the same instructions as before CAUSAL existed.
+#define DSB_AT_UNIT(u)                                                                                                           \
+  const int bh = CAUSAL ? (u) % (p.n_units / p.n_pairs) : (u) / p.n_pairs,                                                       \
+            pair = CAUSAL ? p.n_pairs - 1 - (u) / (p.n_units / p.n_pairs) : (u) - bh * p.n_pairs, b = bh / p.H, h = bh - b * p.H; \
+  const int n_stream = CAUSAL ? min(p.n_chunks, 2 * pair + 2) : p.n_chunks
+
+template <int HD, bool CAUSAL>
 __global__ void __launch_bounds__(AtCfg<HD>::THREADS, 1)
 attention_tc_split_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k, const __grid_constant__ CUtensorMap map_v,
                           const __grid_constant__ AtParams p) {
@@ -234,7 +258,7 @@ attention_tc_split_kernel(const __grid_constant__ CUtensorMap map_q, const __gri
       int stage = 0, qn[2] = {0, 0};
       uint32_t phase = 0;
       for (int u = blockIdx.x; u < p.n_units; u += gridDim.x) {
-        const int bh = u / p.n_pairs, pair = u - bh * p.n_pairs, b = bh / p.H, h = bh - b * p.H;
+        DSB_AT_UNIT(u);
 #pragma unroll
         for (int w = 0; w < 2; ++w) {
           const int tile = 2 * pair + w;
@@ -247,7 +271,7 @@ attention_tc_split_kernel(const __grid_constant__ CUtensorMap map_q, const __gri
           tma_load_3d(&map_q, &q_full[q], dst + C::TILE, p.q_lo_col + h * HD, tile * 64, b);
           ++qn[w];
         }
-        for (int c = 0; c < p.n_chunks; ++c) {
+        for (int c = 0; c < n_stream; ++c) {
           mbar_wait(&empty[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full[stage], C::STAGE_BYTES);
           uint8_t* st = ring + stage * C::STAGE_BYTES;
@@ -266,18 +290,25 @@ attention_tc_split_kernel(const __grid_constant__ CUtensorMap map_q, const __gri
     int stage = 0, qn = 0;
     uint32_t phase = 0;
     for (int u = blockIdx.x; u < p.n_units; u += gridDim.x) {
-      const int bh = u / p.n_pairs, pair = u - bh * p.n_pairs, b = bh / p.H, h = bh - b * p.H;
+      DSB_AT_UNIT(u);
       const int tile = 2 * pair + wg;
       if (tile < p.n_tiles) {
         const int q = 2 * wg + (qn & 1);
         mbar_wait(&q_full[q], (qn >> 1) & 1);
-        at_tile<HD>(p, ring, full, empty, stage, phase, qbuf + q * C::Q_BYTES, b, h, tile, wg, wq, lane);
+        at_tile<HD, CAUSAL>(p, ring, full, empty, stage, phase, qbuf + q * C::Q_BYTES, b, h, tile, wg, wq, lane);
         __syncwarp();
         if (lane == 0) mbar_arrive(&q_empty[q]);
         ++qn;
+        if constexpr (CAUSAL) {
+          for (int c = tile + 1; c < n_stream; ++c) {  // the pair's odd tile's diagonal chunk: released unread by the even tile
+            mbar_wait(&full[stage], phase);
+            if (lane == 0) mbar_arrive(&empty[stage]);
+            if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+          }
+        }
       } else {
         // the odd last tile of a head: this warpgroup only passes the chunks on (waiting for each, so it never runs a ring lap ahead)
-        for (int c = 0; c < p.n_chunks; ++c) {
+        for (int c = 0; c < n_stream; ++c) {
           mbar_wait(&full[stage], phase);
           if (lane == 0) mbar_arrive(&empty[stage]);
           if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
@@ -287,13 +318,17 @@ attention_tc_split_kernel(const __grid_constant__ CUtensorMap map_q, const __gri
   }
 }
 
-// Host side of dsb_attention_tc_split (HD 64) and dsb_attention_tc_split_hd32 (HD 32); `name` prefixes every error message.
-template <int HD>
+#undef DSB_AT_UNIT
+
+// Host side of dsb_attention_tc_split (HD 64), dsb_attention_tc_split_hd32 (HD 32) and dsb_attention_tc_split_causal (both, CAUSAL);
+// `name` prefixes every error message.
+template <int HD, bool CAUSAL = false>
 int attention_tc_split_launch(const char* name, const void* q, long long ldq, long long q_lo_off, const void* k, long long ldk, long long k_lo_off,
                               const void* v, long long ldv, long long v_lo_off, void* o, long long ldo, long long o_lo_off, int B, int H, int Lq,
                               int Lk, float scale, void* stream) {
   using C = AtCfg<HD>;
   DSB_REQUIRE(B > 0 && H > 0 && Lq > 0 && Lk > 0, "%s: need B, H, Lq, Lk > 0", name);
+  DSB_REQUIRE(!CAUSAL || Lq == Lk, "%s: causal attention needs Lq == Lk (got %d, %d)", name, Lq, Lk);
   DSB_REQUIRE(ldo % 8 == 0 && o_lo_off % 8 == 0 && (reinterpret_cast<uintptr_t>(o) & 15) == 0, "%s: o must be 16-byte aligned, ldo / o_lo_off %% 8 == 0",
               name);
   DSB_REQUIRE(q_lo_off >= (long long)H * HD && k_lo_off >= (long long)H * HD && v_lo_off >= (long long)H * HD && o_lo_off >= (long long)H * HD,
@@ -321,11 +356,11 @@ int attention_tc_split_launch(const char* name, const void* q, long long ldq, lo
   if (make_operand_map(&mv, v, DSB_DTYPE_F16, v_lo_off + (long long)H * HD, Lk, B, ldv, (long long)Lk * ldv, 64, 0, C::ROW)) return 3;
   static bool attr_set = false;
   if (!attr_set) {
-    DSB_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_split_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
+    DSB_CHECK_CUDA(cudaFuncSetAttribute(attention_tc_split_kernel<HD, CAUSAL>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
     attr_set = true;
   }
   const int grid = min(p.n_units, sm_count());
-  DSB_CHECK_CUDA(launch_pdl(attention_tc_split_kernel<HD>, dim3(grid), dim3(C::THREADS), C::SMEM, (cudaStream_t)stream, mq, mk, mv, p));
+  DSB_CHECK_CUDA(launch_pdl(attention_tc_split_kernel<HD, CAUSAL>, dim3(grid), dim3(C::THREADS), C::SMEM, (cudaStream_t)stream, mq, mk, mv, p));
   return 0;
 }
 }  // namespace

@@ -1,11 +1,12 @@
 """Drop-in for Codebook/specvqgan/models/cond_transformer.py::Net2NetTransformer, the autoregressive SpecVQGAN baseline (the caps_transformer*.yaml
 configs): same constructor arguments and state_dict keys (`transformer.*`, `first_stage_model.*`, the permuter buffers), the same `forward`,
-`sample`, `encode_to_z`, `encode_to_c`, `decode_to_img` and `top_k_logits`.
+`sample`, `encode_to_z`, `encode_to_c`, `decode_to_img`, `top_k_logits`, `get_input`, `get_xc`, `shared_step` and `validation_step`.
 
 `sample` runs the KV-cached decode of `GPTFeats` (ar_engine.py): one fixed launch sequence per position, replayed from a CUDA graph, with the
 top-k / softmax / multinomial step in-kernel (torch.multinomial(probs, 1)'s CUDA draw replayed from the default CUDA generator, which is left
-where the reference leaves it).  Attention maps are not materialised: `sample` returns (x, None) where the reference returns (x, att).  Training
-(`shared_step`, `configure_optimizers`, pkeep < 1 corruption) and the pkeep <= 0 single-pass branch are not implemented.
+where the reference leaves it).  Attention maps are not materialised: `sample` returns (x, None) where the reference returns (x, att).
+`shared_step` / `validation_step` score a batch (the validation loss) with one causal pass of `GPTFeats.forward_loss`, in eval mode only.
+Training (`training_step`, `configure_optimizers`, pkeep < 1 corruption) and the pkeep <= 0 single-pass branch are not implemented.
 """
 import torch
 from torch import nn
@@ -83,6 +84,48 @@ class Net2NetTransformer(nn.Module):
             return x, None
         ids, _ = tr.sample_tokens(x, c, steps, temperature=temperature, sample=sample, top_k=top_k, callback=callback)
         return ids, None
+
+    def get_input(self, key, batch):
+        """cond_transformer.py:318-335 for string keys: 'feature' / 'target' through the condition stage ((B, Tc, Cf) -> (B, Cf, Tc)), anything else
+        (a mel (B, H, W) or (B, H, W, C)) to (B, C, H, W); doubles become floats."""
+        if not isinstance(key, str):
+            raise NotImplementedError("get_input: only string batch keys are implemented (the caps configs' 'image' / 'feature')")
+        if key in ["feature", "target"]:
+            x = self.cond_stage_model.get_input(batch, key)
+        else:
+            x = batch[key]
+            if len(x.shape) == 3:
+                x = x[..., None]
+            x = x.permute(0, 3, 1, 2).to(memory_format=torch.contiguous_format)
+        if x.dtype == torch.double:
+            x = x.float()
+        return x
+
+    def get_xc(self, batch, N=None):
+        """cond_transformer.py:337-351."""
+        x = self.get_input(self.first_stage_key, batch)
+        c = self.get_input(self.cond_stage_key, batch)
+        if N is not None:
+            x, c = x[:N], c[:N]
+        return x, c
+
+    @torch.no_grad()
+    def shared_step(self, batch, batch_idx=None):
+        """cond_transformer.py:353-360 in eval mode: z = encode_to_z(mel), logits of z[:, :-1] after the condition from row cond_size - 1 on,
+        loss = F.cross_entropy(logits.reshape(-1, V), z.reshape(-1)), from one causal pass.  Returns the loss (0-dim fp32 tensor)."""
+        if self.training:
+            raise NotImplementedError("Net2NetTransformer.shared_step in training mode: only the forward (the loss) is implemented; training "
+                                      "(gradients) is not. Call .eval() to score.")
+        x, c = self.get_xc(batch)
+        x, c = x.to(self.transformer.head.weight.device), c.to(self.transformer.head.weight.device)
+        _, z_indices = self.encode_to_z(x)
+        _, c = self.encode_to_c(c)
+        _, loss, _ = self._feats_transformer().forward_loss(z_indices[:, :-1], c, z_indices, c.size(-1) - 1)
+        return loss
+
+    def validation_step(self, batch, batch_idx=None):
+        """cond_transformer.py:367-370: the shared_step loss (`val/loss`; logging is left to the caller)."""
+        return self.shared_step(batch, batch_idx)
 
     @torch.no_grad()
     def encode_to_z(self, x):

@@ -2,9 +2,10 @@
 Net2NetTransformer samples token by token.  Same constructor arguments, the same parameter / buffer names (a reference checkpoint's
 state_dict loads unchanged, including blocks.N.attn.mask) and the same seeded initialisation order.
 
-The modules hold the parameters; compute runs in `AREngine` (ar_engine.py): a KV-cached decode with CUDA kernels, teacher-forced or sampling.
-Attention maps are not materialised: forward() returns (logits, None, None) where the reference returns (logits, loss, att).  Targets (the
-training loss), embedders other than Conv1d(kernel_size=1) and n_unmasked > 0 are not implemented.
+The modules hold the parameters; compute runs in `AREngine` (ar_engine.py): a KV-cached decode with CUDA kernels, teacher-forced or sampling,
+and a full-sequence causal pass that scores given targets.  Attention maps are not materialised: forward() returns (logits, loss, None) where the
+reference returns (logits, loss, att).  Only the forward is implemented: training (gradients), embedders other than Conv1d(kernel_size=1) and
+n_unmasked > 0 are not.
 """
 from __future__ import annotations
 
@@ -118,18 +119,30 @@ class GPT(nn.Module):
         if self.head.weight.device.type != "cuda":
             raise RuntimeError("the autoregressive transformer runs on CUDA only (no CPU fallback): move the module to a CUDA device")
 
+    def _refuse_training(self, what):
+        if self.training:
+            raise NotImplementedError(f"{what} in training mode: only the forward (logits and loss) is implemented; training (gradients) is not. "
+                                      "Call .eval() to score.")
+
     @torch.no_grad()
     def forward(self, idx, embeddings=None, targets=None):
-        """Teacher-forced logits of every position (B, Tc + n, V) for idx (B, n) after `embeddings` (B, Tc, D).  Returns (logits, None, None):
-        the loss needs `targets` (training, not implemented) and attention maps are not materialised."""
-        if targets is not None:
-            raise NotImplementedError("the training loss (targets) is not implemented")
+        """Logits of every position (B, Tc + n, V) for idx (B, n) after `embeddings` (B, Tc, D).  Without targets: (logits, None, None) from the
+        teacher-forced KV-cached decode (the logits sample() sees).  With targets (B, Tc + n) int64 (ignore_index -100): (logits, loss, None)
+        from one causal pass, loss = F.cross_entropy(logits.view(-1, V), targets.view(-1)) (mingpt.py:183-185); eval mode only.  Attention maps
+        are not materialised."""
         Tc = 0 if embeddings is None else embeddings.shape[1]
         n_pos = Tc + idx.shape[1]
+        if targets is not None:
+            self._refuse_training("GPT.forward with targets")
+            if tuple(targets.shape) != (idx.shape[0], n_pos):
+                raise ValueError(f"targets {tuple(targets.shape)} must be (B, T) = {(idx.shape[0], n_pos)}")
         self._check(n_pos)
         B = idx.shape[0]
         if embeddings is None:
             embeddings = torch.zeros(B, 0, self.config.n_embd, device=idx.device)
+        if targets is not None:
+            logits, loss, _ = self.engine.prefill(embeddings.float(), idx, targets, first_row=0)
+            return logits, loss, None
         _, logits = self.engine.run(embeddings.float(), idx, n_pos, n_pos, record_logits=True)
         return logits, None, None
 
@@ -158,6 +171,20 @@ class GPTFeats(GPT):
         self._check_embedder()
         self._check(feats.shape[-1] + idx.shape[1])
         return super().forward(idx, embeddings=self.engine.embed_condition(feats))
+
+    @torch.no_grad()
+    def forward_loss(self, idx, feats, targets, first_row):
+        """Net2NetTransformer.shared_step's scoring in one causal pass: logits of GPTFeats.forward(idx (B, n), feats (B, Cf, Tc)) from row
+        `first_row` on, and F.cross_entropy of those rows against targets (B, T - first_row) (cond_transformer.py:106, :359).  Returns (logits
+        (B, T - first_row, V), loss (), per-row NLL (B, T - first_row))."""
+        self._refuse_training("Net2NetTransformer.shared_step")
+        self._check_embedder()
+        T = feats.shape[-1] + idx.shape[1]
+        if tuple(targets.shape) != (idx.shape[0], T - first_row):
+            raise ValueError(f"targets {tuple(targets.shape)} must be (B, T - first_row) = {(idx.shape[0], T - first_row)}")
+        self._check(T)
+        logits, loss, nll = self.engine.prefill(self.engine.embed_condition(feats), idx, targets, first_row=first_row)
+        return logits[:, first_row:], loss, nll
 
     @torch.no_grad()
     def sample_tokens(self, x, feats, steps, *, temperature=1.0, sample=False, top_k=None, callback=None, record_logits=False):

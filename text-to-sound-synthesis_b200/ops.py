@@ -385,6 +385,19 @@ def attention_tc_split(q, k, v, out, *, q_lo, k_lo, v_lo, o_lo, B, H, Lq, Lk, sc
     return out
 
 
+def attention_tc_split_causal(q, k, v, out, *, q_lo, k_lo, v_lo, o_lo, B, H, L, scale, head_dim=64):
+    """Causal attention_tc_split (mingpt.py CausalSelfAttention, n_unmasked = 0): query row i of a sequence of L rows attends to keys 0 ... i.
+    Same pair layout and arguments as attention_tc_split with Lq = Lk = L; head_dim 64 or 32."""
+    _attention_head_dim("attention_tc_split_causal", head_dim)
+    _need_cuda(q, k, v, out)
+    if not all(t_.dtype == torch.float16 and t_.stride(-1) == 1 for t_ in (q, k, v, out)):
+        raise RuntimeError("attention_tc_split_causal needs fp16 tensors contiguous in the head dimension")
+    _lib.check(_lib.lib().dsb_attention_tc_split_causal(q.data_ptr(), q.stride(0), q_lo, k.data_ptr(), k.stride(0), k_lo, v.data_ptr(), v.stride(0), v_lo,
+                                                        out.data_ptr(), out.stride(0), o_lo, B, H, L, L, scale, head_dim, _stream()),
+               "dsb_attention_tc_split_causal")
+    return out
+
+
 def posterior_sample(inp, x_t, t, uniform, sched, *, T, trunc_mode=1, trunc_r=0.85, trunc_k=0, t_post=None, x_next=None, log_prob_out=None,
                      stage=0):
     """Fused p_sample tail (see dsb_posterior_sample).  inp: raw logits (B,L,K) fp32, or (B,K+1,L) log-probs with STAGE_INPUT_LOGPROB;
@@ -632,6 +645,42 @@ def ar_embed(cond, tok_emb, pos_emb, ids, x, ctrl, *, err_flag=None):
     _lib.check(_lib.lib().dsb_ar_embed(cond.data_ptr(), tok_emb.data_ptr(), pos_emb.data_ptr(), ids.data_ptr(), ids.stride(0), x.data_ptr(), ctrl.data_ptr(),
                                        B, Tc, tok_emb.shape[0], D, _ptr(err_flag), _stream()), "dsb_ar_embed")
     return x
+
+
+def ar_embed_all(cond, tok_emb, pos_emb, ids, x, *, err_flag=None):
+    """x (B, T, D) = every position's embedding: cond (B, Tc, D) rows first, then tok_emb[ids (B, T - Tc)], plus pos_emb[:T]."""
+    _need_cuda(cond, tok_emb, pos_emb, ids, x, err_flag)
+    B, Tc, D = cond.shape
+    T = x.shape[1]
+    if ids.shape != (B, T - Tc) or x.shape != (B, T, D) or not x.is_contiguous():
+        raise RuntimeError(f"ar_embed_all: ids {tuple(ids.shape)} / x {tuple(x.shape)} do not match cond {tuple(cond.shape)}")
+    _lib.check(_lib.lib().dsb_ar_embed_all(cond.data_ptr(), tok_emb.data_ptr(), pos_emb.data_ptr(), ids.data_ptr(), ids.stride(0), x.data_ptr(), B, T, Tc,
+                                           tok_emb.shape[0], D, _ptr(err_flag), _stream()), "dsb_ar_embed_all")
+    return x
+
+
+def ar_cross_entropy(logits, targets, *, first_row=0, nll=None, loss=None, err_flag=None):
+    """F.cross_entropy (ignore_index -100) of logits (B, T, V) rows first_row ... first_row + n - 1 against targets (B, n) int64.  Returns (loss (),
+    nll (B, n)): the mean over non-ignored rows (NaN if none) and the per-row NLL (0 where ignored).  An out-of-range target sets err_flag, or
+    raises IndexError when no err_flag is given (one 4-byte read)."""
+    _need_cuda(logits, targets, nll, loss, err_flag)
+    B, T, V = logits.shape
+    n = targets.shape[1]
+    if logits.dtype != torch.float32 or logits.stride(2) != 1 or logits.stride(0) != T * logits.stride(1) or targets.dtype != torch.int64 \
+            or targets.stride(1) != 1 or targets.shape[0] != B:
+        raise RuntimeError("ar_cross_entropy: fp32 logits (B, T, V) with uniform row stride and int64 targets (B, n)")
+    if V > AR_MAX_V:
+        raise ValueError(f"ar_cross_entropy: vocabulary of {V} exceeds {AR_MAX_V}")
+    if not 0 <= first_row <= T - n:
+        raise ValueError(f"ar_cross_entropy: rows {first_row} ... {first_row + n - 1} outside the {T} positions")
+    nll = torch.empty(B, n, dtype=torch.float32, device=logits.device) if nll is None else nll
+    loss = torch.empty((), dtype=torch.float32, device=logits.device) if loss is None else loss
+    err = err_flag if err_flag is not None else torch.zeros(1, dtype=torch.int32, device=logits.device)
+    _lib.check(_lib.lib().dsb_ar_cross_entropy(logits.data_ptr(), logits.stride(1), T, int(first_row), n, targets.data_ptr(), targets.stride(0),
+                                               nll.data_ptr(), loss.data_ptr(), B, V, err.data_ptr(), _stream()), "dsb_ar_cross_entropy")
+    if err_flag is None and int(err.item()):
+        raise IndexError(f"Target out of bounds: a target outside [0, {V}) that is not ignore_index (-100)")
+    return loss, nll
 
 
 def ar_attention(qkv, k_cache, v_cache, out, ctrl, *, H, scale, lo_off=None):
