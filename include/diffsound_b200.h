@@ -479,6 +479,54 @@ int dsb_attention_train_bwd(const void* q, long long ldq, const void* k, long lo
 int dsb_embed_bwd(const int64_t* ids, const float* dx, float* demb, float* dheight, float* dwidth, int B, int L, int D, int H, int W,
                   int num_embed, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * ACT audio captioning (reference Codebook/AudiocaptionLoss: models/TransModel.py ACT, models/AudioTransformer.py AudioTransformer_80,
+ * tools/utils.py greedy_decode, tools/beam.py beam_decode).  The encoder's GEMMs, LayerNorms, attention and GELU are the existing split-fp16
+ * entry points; the decoder runs one step for R rows, each row one search node of its own clip.
+ *
+ * Self-attention K / V pool (dsb_caption_tree_attention): per decoder layer two fp32 arrays k_pool / v_pool of n_slots rows, slot s at
+ * s * pool_ld, columns [64 h, 64 h + 64) for head h.  Each expanded node owns one slot (the same slot index in every layer).  The engine gives
+ * clip c the slots [c * S, (c + 1) * S): greedy decoding puts position p at c * S + p, beam search gives the clip's k-th expanded node
+ * c * S + k.  A row's path is the int32 slot list path[path_start[r] ... path_start[r] + pos[r]], its ancestors from the root down, ending
+ * with its own slot.
+ * ------------------------------------------------------------------------------------------------------------- */
+/* AudioTransformer_80.forward (AudioTransformer.py:212-219): x = bn0(spec) in eval mode, then patch_embed's Rearrange with (p1, p2) = (4, 80),
+ * which is a reshape of each clip's (T, 80) rows into (T / 4, 320).  spec (B, T, 80) fp32 (clip stride spec_bs) -> out (B * T / 4, 640) fp16
+ * [hi(320) | lo(320)] of y = x * alpha[f] + beta[f] (alpha = weight / sqrt(running_var + eps), beta = bias - running_mean * alpha, per mel
+ * bin f).  T % 4 == 0. */
+int dsb_caption_frontend(const float* spec, long long spec_bs, int B, int T, const float* alpha, const float* beta, void* out, void* stream);
+/* AudioTransformer.py:223-229: x = cat(cls_token, patches) + pos_embedding[:, :n + 1].  patch (B * n, D), cls (D), pos (>= n + 1, D) ->
+ * x (B, n + 1, D), fp32. */
+int dsb_caption_tokens(const float* patch, const float* cls, const float* pos, float* x, int B, int n, int D, void* stream);
+/* ACT.decode's embedding for one position per row (TransModel.py:136-137): x[r] = table[tok[r]] + pe[pos[r]] with table = word_emb *
+ * sqrt(nhid) packed once, the reference's fp32 emb * sqrt(d) + pe[p].  A token outside [0, V) or a position outside [0, max_pos) sets
+ * *err_flag and reads row 0.  Replaces the decode's prefix re-embedding. */
+int dsb_caption_embed(const int64_t* tok, const int* pos, const float* table, const float* pe, float* x, int R, int V, int D, int max_pos,
+                      int* err_flag, void* stream);
+/* nn.TransformerDecoderLayer.self_attn under generate_square_subsequent_mask for the last position of each row's prefix (TransModel.py:139-142,
+ * beam.py:108), per (head, row): writes K / V of qkv row r (fp32 (R, 3D) [Q | K | V]) into the row's own slot (the last of its path), then
+ * attends over the pos[r] + 1 path slots in fp32 with a fixed order: s_j = (q . k_j, lane pairs then xor butterfly) * scale, softmax with
+ * expf, o = sum_j p_j v_j.  o is written as the fp16 (hi | lo) pair of out_proj's A operand (hi at out[r * ld_out + c], lo lo_off halves
+ * further).  head_dim 64; max_len (<= 16384) sizes shared memory.  A row whose pos[r] + 1 is outside [1, max_len], whose slot list
+ * leaves the path_len entries of path, or whose path names a slot outside [0, n_slots) sets *err_flag and writes nothing. */
+int dsb_caption_tree_attention(const float* qkv, long long ld_qkv, float* k_pool, float* v_pool, long long pool_ld, long long n_slots, const int* path,
+                               long long path_len, const long long* path_start, const int* pos, int max_len, void* out, long long ld_out,
+                               long long lo_off, int R, int H, int head_dim, float scale, int* err_flag, void* stream);
+/* nn.TransformerDecoderLayer.multihead_attn over the encoder memory (memory_mask None), per (head, row): query q row r (fp32) against the Lm
+ * memory rows of clip row_clip[r], K at kv + (c * Lm + j) * ld_kv (projected once per batch), V v_off further; the same fp32 order and pair
+ * output as dsb_caption_tree_attention.  head_dim 64, Lm <= 16384.  A row whose clip is outside [0, n_clips) sets *err_flag and writes
+ * nothing. */
+int dsb_caption_cross_attention(const float* q, long long ldq, const float* kv, long long ld_kv, long long v_off, int Lm, const int* row_clip,
+                                int n_clips, void* out, long long ld_out, long long lo_off, int R, int H, int head_dim, float scale, int* err_flag,
+                                void* stream);
+/* The choice after dec_fc, one CTA per row, V <= 16384:
+ *   k_top > 0: F.log_softmax then torch.topk(log_prob, k_top) (beam.py:109-112): vals / idx (R, k_top), descending, ties to the lowest index.
+ *   k_top = 0: argmax(F.softmax(logits)) (utils.py:87-88), ties to the lowest index -> ys[r * ys_ld + pos[r] + 1] and tok[r]; pos[r] += 1, so
+ *   the next step's embed and self-attention read the advanced position (a captured step replays for every position).
+ * k_top <= 16.  A NaN or infinite logit sets *err_flag. */
+int dsb_caption_select(const float* logits, long long ld, int R, int V, int k_top, float* vals, int64_t* idx, int64_t* ys, long long ys_ld, int64_t* tok,
+                       int* pos, int* err_flag, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

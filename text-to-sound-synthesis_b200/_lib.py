@@ -85,6 +85,13 @@ SIGNATURES = {
     "dsb_pair_maxpool3s2": [c_vp] + [c_i] * 6 + [c_vp, c_ll, c_ll] + [c_i] * 6 + [c_f, c_vp],
     "dsb_pair_avgpool3": [c_vp] + [c_i] * 6 + [c_vp, c_ll, c_ll, c_i, c_i, c_vp],
     "dsb_pair_channel_mean": [c_vp, c_ll, c_ll] + [c_i] * 8 + [c_f, c_vp, c_vp],
+    # ACT audio captioning
+    "dsb_caption_frontend": [c_vp, c_ll, c_i, c_i, c_vp, c_vp, c_vp, c_vp],
+    "dsb_caption_tokens": [c_vp] * 4 + [c_i] * 3 + [c_vp],
+    "dsb_caption_embed": [c_vp] * 5 + [c_i] * 4 + [c_vp, c_vp],
+    "dsb_caption_tree_attention": [c_vp, c_ll, c_vp, c_vp, c_ll, c_ll, c_vp, c_ll, c_vp, c_vp, c_i, c_vp, c_ll, c_ll, c_i, c_i, c_i, c_f, c_vp, c_vp],
+    "dsb_caption_cross_attention": [c_vp, c_ll, c_vp, c_ll, c_ll, c_i, c_vp, c_i, c_vp, c_ll, c_ll, c_i, c_i, c_i, c_f, c_vp, c_vp],
+    "dsb_caption_select": [c_vp, c_ll, c_i, c_i, c_i, c_vp, c_vp, c_vp, c_ll, c_vp, c_vp, c_vp, c_vp],
     # SpecVQGAN log-mel spectrogram
     "dsb_wav_frames_f16": [c_vp, c_ll, c_i, c_i, c_vp, c_i, c_vp, c_vp],
     "dsb_mel_log": [c_vp, c_ll, c_ll] + [c_i] * 4 + [c_vp] * 3 + [c_i, c_i, c_vp, c_vp],

@@ -767,3 +767,101 @@ def mel_log(spec, n_bins, fb_start, fb_len, fb_w, T_out, out=None):
     _lib.check(_lib.lib().dsb_mel_log(spec.data_ptr(), ld, spec.stride(0), B, T, T_out, n_bins, fb_start.data_ptr(), fb_len.data_ptr(), fb_w.data_ptr(),
                                       fb_ld, n_mels, out.data_ptr(), _stream()), "dsb_mel_log")
     return out
+
+
+# ---------------------------------------------------------------- ACT audio captioning (caption.cu)
+CAPTION_MAX_V = 16384
+CAPTION_MAX_LEN = 16384
+CAPTION_MAX_K = 16
+CAPTION_HEAD_DIM = 64
+
+
+def caption_frontend(spec, alpha, beta, out=None):
+    """spec (B, T, 80) fp32 -> (B * T / 4, 640) fp16 pair of the BatchNorm eval affine x * alpha[f] + beta[f], as 4 x 80 patch rows."""
+    _need_cuda(spec, alpha, beta, out)
+    B, T, F = spec.shape
+    if F != 80 or T % 4 or spec.stride(2) != 1 or spec.stride(1) != 80 or spec.dtype != torch.float32:
+        raise RuntimeError(f"caption_frontend: fp32 (B, T, 80) spectrogram with T % 4 == 0 and contiguous frames, got {tuple(spec.shape)}")
+    if out is None:
+        out = torch.empty(B * (T // 4), 640, dtype=torch.float16, device=spec.device)
+    _lib.check(_lib.lib().dsb_caption_frontend(spec.data_ptr(), spec.stride(0), B, T, alpha.data_ptr(), beta.data_ptr(), out.data_ptr(), _stream()),
+               "dsb_caption_frontend")
+    return out
+
+
+def caption_tokens(patch, cls, pos, x):
+    """x (B, n + 1, D) = cat(cls, patch (B * n, D)) + pos[:n + 1]."""
+    _need_cuda(patch, cls, pos, x)
+    B, L, D = x.shape
+    _lib.check(_lib.lib().dsb_caption_tokens(patch.data_ptr(), cls.data_ptr(), pos.data_ptr(), x.data_ptr(), B, L - 1, D, _stream()), "dsb_caption_tokens")
+    return x
+
+
+def caption_embed(tok, pos, table, pe, x, *, err_flag=None):
+    """x (R, D) = table[tok (R,) int64] + pe[pos (R,) int32]."""
+    _need_cuda(tok, pos, table, pe, x, err_flag)
+    R, D = x.shape
+    _lib.check(_lib.lib().dsb_caption_embed(tok.data_ptr(), pos.data_ptr(), table.data_ptr(), pe.data_ptr(), x.data_ptr(), R, table.shape[0], D, pe.shape[0],
+                                            _ptr(err_flag), _stream()), "dsb_caption_embed")
+    return x
+
+
+def caption_tree_attention(qkv, k_pool, v_pool, path, path_start, pos, out, *, R, H, scale, max_len, lo_off=None, err_flag=None):
+    """Tree self-attention (see dsb_caption_tree_attention): qkv (>= R, 3D) fp32, pools (n_slots, D) fp32, path int32, path_start (R,) int64,
+    pos (R,) int32, out the fp16 pair (R, 2D).  A path that does not fit max_len, path or the pool sets err_flag (int32) and is skipped."""
+    _need_cuda(qkv, k_pool, v_pool, path, path_start, pos, out, err_flag)
+    D = k_pool.shape[1]
+    if D != H * CAPTION_HEAD_DIM:
+        raise ValueError(f"caption_tree_attention: head_dim {D / H} unsupported ({CAPTION_HEAD_DIM})")
+    if max_len > CAPTION_MAX_LEN:
+        raise ValueError(f"caption_tree_attention: a path of {max_len} nodes exceeds {CAPTION_MAX_LEN}")
+    if path.dtype != torch.int32 or path_start.dtype != torch.int64 or pos.dtype != torch.int32 or k_pool.stride(1) != 1 or v_pool.stride() != k_pool.stride():
+        raise RuntimeError("caption_tree_attention: int32 path / pos, int64 path_start, pools with one row stride")
+    _lib.check(_lib.lib().dsb_caption_tree_attention(qkv.data_ptr(), qkv.stride(0), k_pool.data_ptr(), v_pool.data_ptr(), k_pool.stride(0),
+                                                     min(k_pool.shape[0], v_pool.shape[0]), path.data_ptr(), path.numel(), path_start.data_ptr(),
+                                                     pos.data_ptr(), int(max_len), out.data_ptr(), out.stride(0), D if lo_off is None else lo_off, R, H,
+                                                     CAPTION_HEAD_DIM, float(scale), _ptr(err_flag), _stream()),
+               "dsb_caption_tree_attention")
+    return out
+
+
+def caption_cross_attention(q, kv, row_clip, out, *, R, H, Lm, v_off, scale, lo_off=None, err_flag=None):
+    """Cross-attention (see dsb_caption_cross_attention): q (>= R, D) fp32, kv a row-strided fp32 view whose row c * Lm + j holds clip c's key j
+    (value v_off further), row_clip (R,) int32, out the fp16 pair (R, 2D).  A clip outside the kv.shape[0] // Lm clips sets err_flag and is
+    skipped."""
+    _need_cuda(q, kv, row_clip, out, err_flag)
+    D = H * CAPTION_HEAD_DIM
+    if row_clip.dtype != torch.int32 or q.dtype != torch.float32 or kv.dtype != torch.float32:
+        raise RuntimeError("caption_cross_attention: fp32 q / kv and int32 row_clip")
+    if kv.stride(1) != 1 or v_off + D > kv.shape[1] or kv.shape[0] < Lm:
+        raise RuntimeError(f"caption_cross_attention: kv {tuple(kv.shape)} holds no (K | V) rows of width {D} at v_off {v_off}")
+    _lib.check(_lib.lib().dsb_caption_cross_attention(q.data_ptr(), q.stride(0), kv.data_ptr(), kv.stride(0), int(v_off), int(Lm), row_clip.data_ptr(),
+                                                      kv.shape[0] // Lm, out.data_ptr(), out.stride(0), D if lo_off is None else lo_off, R, H,
+                                                      CAPTION_HEAD_DIM, float(scale), _ptr(err_flag), _stream()), "dsb_caption_cross_attention")
+    return out
+
+
+def caption_select_topk(logits, k, vals, idx, *, R=None, err_flag=None):
+    """Beam choice: log_softmax of logits rows (R, V), top k values / indices (R, k) in descending order, ties to the lowest index."""
+    _need_cuda(logits, vals, idx, err_flag)
+    R = logits.shape[0] if R is None else R
+    V = logits.shape[1]
+    check_caption_vocab(V)
+    _lib.check(_lib.lib().dsb_caption_select(logits.data_ptr(), logits.stride(0), R, V, int(k), vals.data_ptr(), idx.data_ptr(), None, 0, None, None,
+                                             _ptr(err_flag), _stream()), "dsb_caption_select")
+    return vals, idx
+
+
+def caption_select_greedy(logits, ys, tok, pos, *, err_flag=None):
+    """Greedy choice: argmax(softmax(logits row r)) -> ys[r, pos[r] + 1] and tok[r]; pos[r] += 1."""
+    _need_cuda(logits, ys, tok, pos, err_flag)
+    R, V = logits.shape
+    check_caption_vocab(V)
+    _lib.check(_lib.lib().dsb_caption_select(logits.data_ptr(), logits.stride(0), R, V, 0, None, None, ys.data_ptr(), ys.stride(0), tok.data_ptr(),
+                                             pos.data_ptr(), _ptr(err_flag), _stream()), "dsb_caption_select")
+    return ys
+
+
+def check_caption_vocab(V):
+    if V > CAPTION_MAX_V:
+        raise ValueError(f"the caption decoder's select takes a vocabulary of at most {CAPTION_MAX_V} words, got {V}")
