@@ -161,7 +161,7 @@ def test_encoder_full_config_matches_oracle(G):
     cb = zf.mean(0, keepdim=True) + torch.randn(256, 256, generator=g) * zf.std(0, keepdim=True)   # codes with the latents' statistics
     sd["content_codec.quantize.embedding.weight"] = cb
     m.quantize.embedding.weight.data.copy_(cb.cuda())
-    m.enc_engine.packed = False
+    m.enc_engine.repack()
     _, tok_ref = O.encode_to_tokens(sd, mel)
     quant, _, info = m.encode(mel.cuda())
     e_z = rel_err(m.last_latent.cpu(), z_ref)

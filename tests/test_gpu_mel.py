@@ -178,7 +178,7 @@ def test_encoder_tokens_and_reconstruct_on_gpu_mel(G, eng):
     g = torch.Generator().manual_seed(6)
     cb = zf.mean(0, keepdim=True) + torch.randn(256, 256, generator=g) * zf.std(0, keepdim=True)
     m.quantize.embedding.weight.data.copy_(cb.cuda())
-    m.enc_engine.packed = False
+    m.enc_engine.repack()
     _, _, info_ref = m.encode(mel_ref)
     z_ref = m.last_latent.permute(0, 2, 3, 1).reshape(-1, 256).double().cpu()
     _, _, info = m.encode(mel_gpu)

@@ -26,40 +26,26 @@ import numpy as np
 import torch
 
 from . import ops
+from .engine_base import PackedEngine
+from .graphs import capture
 from .packing import SplitWeight
 
 
-class AREngine:
+class AREngine(PackedEngine):
+    settings = ("use_cuda_graph",)
+
     def __init__(self, gpt, use_cuda_graph: bool = True):
-        self.m = gpt
+        super().__init__(gpt, use_cuda_graph=use_cuda_graph)
         self.use_cuda_graph = use_cuda_graph
-        self.packed = False
         self._ws: Dict[int, dict] = {}
         self._pf: Dict[tuple, dict] = {}  # the prefill workspace of the latest (B, T)
-        self.generation = 0  # bumped by repack(): graphs that baked old pointers are rebuilt
-        self._param_sig = None
         self.launches_per_step = 0
-
-    def __deepcopy__(self, memo):
-        """copy.deepcopy(module) gets a fresh, unpacked engine bound to the copied module: packed weights, workspaces, KV caches and captured
-        graphs are per-instance caches, not state."""
-        return AREngine(memo.get(id(self.m), self.m), use_cuda_graph=self.use_cuda_graph)
-
-    def _signature(self):
-        """(storage pointer, in-place version counter) of every parameter: changes on optimizer.step(), p.data.copy_(), .to()."""
-        return tuple((p.data_ptr(), p._version) for p in self.m.parameters())
-
-    def ensure_current(self) -> None:
-        if not self.packed or self._param_sig != self._signature():
-            self.repack()
 
     @property
     def device(self):
         return self.m.head.weight.device
 
-    @torch.no_grad()
-    def repack(self) -> None:
-        """(Re)build packed copies from the module's current parameters."""
+    def _pack(self) -> None:
         m = self.m
         check_ar_shapes(m.config.vocab_size, m.config.n_embd, m.config.n_head, m.block_size)
         if self.device.type != "cuda":
@@ -85,9 +71,6 @@ class AREngine:
         if emb is not None:
             self.wc = f(emb.weight.reshape(emb.weight.shape[0], -1))
             self.bc = f(emb.bias) if emb.bias is not None else None
-        self._param_sig = self._signature()
-        self.packed = True
-        self.generation += 1
         self._ws.clear()
         self._pf.clear()
 
@@ -174,21 +157,9 @@ class AREngine:
             ws["ids"][:, :n_given].copy_(ids)
         key = (Tc, float(temperature), top_k, bool(sample), record_logits)
         g = ws["graphs"].get(key) if self.use_cuda_graph else None
-        if g is not None and g[1] != self.generation:
-            g = None
-        if self.use_cuda_graph and g is None:
-            # warm-up on a side stream (lazy inits), then capture one step; the loop state is re-armed afterwards
+        if self.use_cuda_graph and g is None:  # the warm-up runs one step: the loop state is re-armed afterwards
             self._arm(ws, seed, offset, counter_offset, nthreads, n_pos, first)
-            s = torch.cuda.Stream(device=dev)
-            s.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(s):
-                self._step(ws, Tc, temperature, top_k, sample, hist)
-            torch.cuda.current_stream(dev).wait_stream(s)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                self._step(ws, Tc, temperature, top_k, sample, hist)
-            g = (graph, self.generation)
-            ws["graphs"][key] = g
+            g = ws["graphs"][key] = capture(lambda: self._step(ws, Tc, temperature, top_k, sample, hist), dev)
         self._arm(ws, seed, offset, counter_offset, nthreads, n_pos, first)
         if n_given:  # the warm-up step may have written a sampled token over the given ones
             ws["ids"][:, :n_given].copy_(ids)
@@ -196,7 +167,7 @@ class AREngine:
             if callback is not None and p >= first:
                 callback(p - first)
             if g is not None:
-                g[0].replay()
+                g.replay()
             else:
                 self._step(ws, Tc, temperature, top_k, sample, hist)
         n_sampled = max(0, n_pos - first)
@@ -272,22 +243,10 @@ class AREngine:
             ws["tgt"][:, :n].copy_(targets)
         key = (Tc, first_row, n)
         g = ws["graphs"].get(key) if self.use_cuda_graph else None
-        if g is not None and g[1] != self.generation:
-            g = None
         if self.use_cuda_graph and g is None:
-            dev = self.device
-            s = torch.cuda.Stream(device=dev)  # warm-up on a side stream (lazy inits), then capture
-            s.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(s):
-                self._prefill_step(ws, B, T, Tc, first_row, n)
-            torch.cuda.current_stream(dev).wait_stream(s)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                self._prefill_step(ws, B, T, Tc, first_row, n)
-            g = (graph, self.generation)
-            ws["graphs"][key] = g
+            g = ws["graphs"][key] = capture(lambda: self._prefill_step(ws, B, T, Tc, first_row, n), self.device)
         if g is not None:
-            g[0].replay()
+            g.replay()
         else:
             self._prefill_step(ws, B, T, Tc, first_row, n)
         err = ws["err"].tolist()  # one 8-byte read per call

@@ -20,6 +20,8 @@ import numpy as np
 import torch
 
 from . import ops
+from .engine_base import PackedEngine
+from .graphs import capture
 from .packing import SplitWeight
 
 MAX_POS = 2000                       # rows of PositionalEncoding.pe: the reference cannot decode a longer prefix
@@ -27,29 +29,21 @@ BEAM_SLOTS = 2002                    # slots per clip in beam search: at most 20
 HEAD_PAD = 528                       # the 527 AudioSet logits padded to a multiple of 4 (16-byte GEMM operand rows)
 
 
-class CaptionEngine:
+class CaptionEngine(PackedEngine):
+    settings = ("use_cuda_graph",)
+
     def __init__(self, act, use_cuda_graph: bool = True):
-        self.m = act
+        super().__init__(act, use_cuda_graph=use_cuda_graph)
         self.use_cuda_graph = use_cuda_graph
-        self.packed = False
-        self._param_sig = None
-        self.generation = 0
         self._enc: Dict[tuple, dict] = {}
         self._dec: Dict[tuple, dict] = {}
-
-    def _signature(self):
-        return tuple((p.data_ptr(), p._version) for p in self.m.parameters()) + tuple((b.data_ptr(), b._version) for b in self.m.buffers())
-
-    def ensure_current(self) -> None:
-        if not self.packed or self._param_sig != self._signature():
-            self.repack()
+        self._last = None  # the encoder workspace of the last encode() / decode memory
 
     @property
     def device(self):
         return self.m.dec_fc.weight.device
 
-    @torch.no_grad()
-    def repack(self) -> None:
+    def _pack(self) -> None:
         m = self.m
         if self.device.type != "cuda":
             raise RuntimeError("CaptionEngine needs the module on a CUDA device (no CPU fallback)")
@@ -105,11 +99,9 @@ class CaptionEngine:
         self.table = (f(m.word_emb.weight) * math.sqrt(m.nhid)).contiguous()  # decode(): self.word_emb(tgt) * math.sqrt(self.nhid), in fp32
         self.pe = f(m.pos_encoder.pe.reshape(m.pos_encoder.pe.shape[0], -1))
         self.w_fc, self.b_fc = SplitWeight(m.dec_fc.weight), f(m.dec_fc.bias)
-        self._param_sig = self._signature()
-        self.packed = True
-        self.generation += 1
         self._enc.clear()
         self._dec.clear()
+        self._last = None
 
     # ------------------------------------------------------------------ encoder
     def _enc_ws(self, B: int, T: int) -> dict:
@@ -154,22 +146,11 @@ class CaptionEngine:
         ops.gemm_f16x3(ws["memp"], self.w_kv.pair, self.b_kv, out=ws["kv"], alpha=self.w_kv.alpha)
 
     def _replay(self, ws, step) -> None:
-        g = ws.get("graph")
-        if self.use_cuda_graph and (g is None or g[1] != self.generation):
-            dev = self.device
-            s = torch.cuda.Stream(device=dev)  # warm-up on a side stream (lazy inits), then capture
-            s.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(s):
-                step()
-            torch.cuda.current_stream(dev).wait_stream(s)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                step()
-            g = ws["graph"] = (graph, self.generation)
-        if self.use_cuda_graph:
-            g[0].replay()
-        else:
-            step()
+        if not self.use_cuda_graph:
+            return step()
+        if ws["graph"] is None:
+            ws["graph"] = capture(step, self.device)
+        ws["graph"].replay()
 
     @torch.no_grad()
     def encode(self, spec: torch.Tensor) -> torch.Tensor:
@@ -188,7 +169,7 @@ class CaptionEngine:
     def _memory_ws(self, memory: torch.Tensor) -> dict:
         """The encoder workspace holding `memory` and its projected K / V: the last encode() when memory is its output, else one filled here."""
         B, Lm, D = memory.shape
-        ws = getattr(self, "_last", None)
+        ws = self._last
         if ws is not None and ws["mem"].shape == memory.shape and torch.equal(ws["mem"], memory):
             return ws
         ws = self._enc_ws(B, 4 * (Lm - 1))
@@ -308,22 +289,13 @@ class CaptionEngine:
 
         key = ("greedy", id(enc["kv"]), max_len)
         g = ws["graphs"].get(key) if self.use_cuda_graph else None
-        if self.use_cuda_graph and (g is None or g[1] != self.generation):
+        if self.use_cuda_graph and g is None:  # the warm-up runs one step: the state is re-armed afterwards
             arm()
-            s = torch.cuda.Stream(device=self.device)
-            s.wait_stream(torch.cuda.current_stream(self.device))
-            with torch.cuda.stream(s):
-                step()
-            torch.cuda.current_stream(self.device).wait_stream(s)
-            arm()
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                step()
-            g = ws["graphs"][key] = (graph, self.generation)
+            g = ws["graphs"][key] = capture(step, self.device)
         arm()
         for _ in range(max_len):
             if g is not None:
-                g[0].replay()
+                g.replay()
             else:
                 step()
         self._check_err(ws)

@@ -11,11 +11,14 @@ from __future__ import annotations
 import torch
 
 from . import ops
+from .engine_base import PackedEngine
 from .graphs import GraphCache
 from .packing import PackedConv
 
 
-class DecoderEngine:
+class DecoderEngine(PackedEngine):
+    settings = ("use_cuda_graph", "max_batch")
+
     def __init__(self, vq, precision: str = "f16x3"):
         """precision: 'f16x3'  -- split-fp16 operands: conv inputs leave GroupNorm / upsample / the codebook gather as fp16 (hi | lo) pairs, weights are
                                    (hi | lo) pairs of 2^s * W, every product is lo*hi + hi*lo + hi*hi on fp16 wgmma with fp32 accumulation:
@@ -25,9 +28,8 @@ class DecoderEngine:
                       'tf32'   -- single-pass TF32 (3x fewer MMAs; mel error ~4e-3 relative)."""
         if precision not in ("f16x3", "tf32x3", "tf32"):
             raise ValueError("precision must be 'f16x3', 'tf32x3' or 'tf32'")
-        self.vq = vq
+        super().__init__(vq, precision=precision)
         self.precision = precision
-        self.packed = False
         self.launches = 0
         self.use_cuda_graph = True
         self.max_batch = 32  # clips per pass: bounds the activation memory (34.7 MB fp32 per clip per full-resolution tensor) at any caller batch
@@ -48,9 +50,8 @@ class DecoderEngine:
             return ops.gemm_split(a if presplit else ops.split_tf32(a), w, bias, residual, out, **kw)
         return ops.gemm(a, w, bias, residual, out, **kw)
 
-    @torch.no_grad()
-    def repack(self):
-        vq, d = self.vq, self.vq.decoder
+    def _pack(self):
+        vq, d = self.m, self.m.decoder
         if vq.post_quant_conv.weight.device.type != "cuda":
             raise RuntimeError("DecoderEngine needs the module on a CUDA device (no CPU fallback)")
         f = lambda p: p.detach().float().contiguous()
@@ -86,7 +87,6 @@ class DecoderEngine:
         gn("norm_out", d.norm_out)
         conv("conv_out", d.conv_out)
         self.codebook = f(vq.quantize.embedding.weight)
-        self.packed = True
         self._graphs.clear()
 
     # ------------------------------------------------------------------ building blocks (all on padded NHWC tensors)
@@ -169,7 +169,7 @@ class DecoderEngine:
     # ------------------------------------------------------------------ entry points
     @torch.no_grad()
     def _decode_padded(self, z):
-        d = self.vq.decoder
+        d = self.m.decoder
         if self.precision == "f16x3":
             z = self._conv(z, "post_quant", pair_out=True)  # 1x1 conv straight into the next conv's (hi | lo) operand: no GroupNorm between them
             h = self._conv(z, "conv_in")
@@ -194,8 +194,7 @@ class DecoderEngine:
 
     @torch.no_grad()
     def decode_tokens(self, ids, grid):
-        if not self.packed:
-            self.repack()
+        self.ensure_current()
         H, W = grid
         ids = ids.contiguous()
         if ids.shape[0] > self.max_batch:
@@ -219,8 +218,7 @@ class DecoderEngine:
     @torch.no_grad()
     def decode_latents(self, quant):
         """quant (B, E, H, W) NCHW (the reference's VQModel.decode input) -> mel; layout conversion is plain data movement."""
-        if not self.packed:
-            self.repack()
+        self.ensure_current()
         self.launches = 1
         z = torch.nn.functional.pad(quant.detach().float().permute(0, 2, 3, 1), (0, 0, 1, 1, 1, 1)).contiguous()
         if self.precision == "f16x3":

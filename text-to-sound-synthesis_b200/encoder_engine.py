@@ -20,10 +20,10 @@ from .decoder_engine import DecoderEngine
 class EncoderEngine(DecoderEngine):
     def __init__(self, vq):
         super().__init__(vq, precision="tf32x3")
+        self.options = {}  # EncoderEngine(vq) takes no arguments of its own
 
-    @torch.no_grad()
-    def repack(self):
-        vq, e = self.vq, self.vq.encoder
+    def _pack(self):
+        vq, e = self.m, self.m.encoder
         if vq.quant_conv.weight.device.type != "cuda":
             raise RuntimeError("EncoderEngine needs the module on a CUDA device (no CPU fallback)")
         f = lambda p: p.detach().float().contiguous()
@@ -61,7 +61,6 @@ class EncoderEngine(DecoderEngine):
         self.codebook = cb
         self.cb_split = ops.pack_split_weight(cb, 1)          # (K, 3*Ep) W operand of the distance GEMM
         self.cb_sq = (cb.double() ** 2).sum(1).float()         # |e_k|^2, set-up time only
-        self.packed = True
         self._graphs.clear()
 
     def _downsample(self, x, name):
@@ -85,7 +84,7 @@ class EncoderEngine(DecoderEngine):
 
     @torch.no_grad()
     def _encode_padded(self, x):
-        e = self.vq.encoder
+        e = self.m.encoder
         h = self._conv(x, "conv_in")
         for lvl in range(e.num_resolutions):
             for j in range(e.num_res_blocks):
@@ -103,10 +102,9 @@ class EncoderEngine(DecoderEngine):
     @torch.no_grad()
     def encode(self, mel):
         """mel (B, 1, H, W) fp32 NCHW -> (z (B, E, H/16, W/16) after quant_conv, nearest-code ids (B, H/16 * W/16) row-major)."""
-        if not self.packed:
-            self.repack()
+        self.ensure_current()
         B, Cin, H, W = mel.shape
-        down = 2 ** (self.vq.encoder.num_resolutions - 1)
+        down = 2 ** (self.m.encoder.num_resolutions - 1)
         if H % down or W % down:
             raise RuntimeError(f"encoder input {H}x{W} must be divisible by {down}")
         self.launches = 0

@@ -11,16 +11,16 @@ What is hoisted relative to the reference (all algebraically identical):
 from __future__ import annotations
 
 import math
-import copy
 from typing import Dict, Optional
 
 import torch
 
 from . import ops
+from .engine_base import PackedEngine
 from .packing import SplitWeight
 
 
-class DenoiserEngine:
+class DenoiserEngine(PackedEngine):
     def __init__(self, transformer, precision: str = "f16x3"):
         """precision: 'f16x3' -- the parity-grade tensor-core mode (default): every GEMM / attention operand is an fp16 (hi | lo) pair
                                 (22 significand bits), products run as three fp16 wgmma passes (lo*hi + hi*lo + hi*hi) into one
@@ -32,27 +32,10 @@ class DenoiserEngine:
                       'fp32'  -- exact FFMA GEMMs (slow; the fp32-exact mode of SURVEY.md section 7.2)."""
         if precision not in ("f16x3", "f16", "tf32", "fp32"):
             raise ValueError("precision must be 'f16x3', 'f16', 'tf32' or 'fp32'")
-        self.m = transformer
+        super().__init__(transformer, precision=precision)
         self.precision = precision
-        self.packed = False
         self._ws: Dict[int, dict] = {}
         self.launches_per_forward = 0
-        self.generation = 0  # bumped by repack(): captured CUDA graphs that baked old pointers must be rebuilt
-        self._param_sig = None
-
-    def __deepcopy__(self, memo):
-        """copy.deepcopy(module) (the reference EMA's shadow model, engine/ema.py:19) gets a fresh, unpacked engine bound to the COPIED module:
-        packed weights, workspaces and anything captured in CUDA graphs are per-instance caches, not state."""
-        return DenoiserEngine(memo.get(id(self.m), self.m), precision=self.precision)
-
-    def _signature(self):
-        """(storage pointer, in-place version counter) of every parameter: changes on optimizer.step(), p.data.copy_(), EMA swaps, .to()."""
-        return tuple((p.data_ptr(), p._version) for p in self.m.parameters())
-
-    def ensure_current(self) -> None:
-        """Repack if the module's parameters changed since the packed copies were made (in-place updates do not go through load_state_dict)."""
-        if not self.packed or self._param_sig != self._signature():
-            self.repack()
 
     # ------------------------------------------------------------------ weights
     @property
@@ -67,9 +50,7 @@ class DenoiserEngine:
             return ops.to_f16(w)
         return ops.round_tf32(w) if self.precision == "tf32" else w.clone()
 
-    @torch.no_grad()
-    def repack(self) -> None:
-        """(Re)build packed copies from the module's current parameters.  Call after load_state_dict / EMA swaps."""
+    def _pack(self) -> None:
         m = self.m
         if self.device.type != "cuda":
             raise RuntimeError("DenoiserEngine needs the module on a CUDA device (no CPU fallback)")
@@ -110,9 +91,6 @@ class DenoiserEngine:
         ce = m.content_emb
         self.emb, self.hemb, self.wemb = f(ce.emb.weight), f(ce.height_emb.weight), f(ce.width_emb.weight)
         self.K = m.to_logits[1].weight.shape[0]
-        self._param_sig = self._signature()
-        self.packed = True
-        self.generation += 1
         self._ws.clear()
 
     def _adaln_table(self, ln) -> torch.Tensor:

@@ -9,6 +9,9 @@ from collections import OrderedDict
 import torch
 import torch.nn as nn
 
+from ...caption_engine import CaptionEngine
+from ...engine_base import EngineModule
+
 NUM_CLASSES, PATCH, EMBED_DIM, DEPTH, HEADS, MLP_DIM = 527, (4, 80), 768, 12, 12, 3072
 
 
@@ -92,7 +95,7 @@ def _cfg(config, *path):
     return config
 
 
-class ACT(nn.Module):
+class ACT(EngineModule):
     """ACT(config, ntoken): the reference's constructor (config.encoder.pretrained loads config.path.encoder, config.word_embedding.pretrained
     needs gensim) and module tree; encode / decode / forward run on the GPU (the module must live on a CUDA device)."""
 
@@ -128,27 +131,7 @@ class ACT(nn.Module):
             self.word_emb.weight.requires_grad = False
         if _cfg(config, "word_embedding", "pretrained"):
             self.word_emb.weight.data = _align_word_embedding(_cfg(config, "path", "vocabulary"), _cfg(config, "path", "word2vec"), self.nhid)
-        self._engine = None
-
-    @property
-    def engine(self):
-        if self._engine is None:
-            from ...caption_engine import CaptionEngine
-            self._engine = CaptionEngine(self)
-        return self._engine
-
-    def __deepcopy__(self, memo):
-        import copy
-        eng, self._engine = self._engine, None
-        try:
-            cls = self.__class__
-            new = cls.__new__(cls)
-            memo[id(self)] = new
-            for k, v in self.__dict__.items():
-                setattr(new, k, copy.deepcopy(v, memo))
-            return new
-        finally:
-            self._engine = eng
+        self.engine = CaptionEngine(self)
 
     def generate_square_subsequent_mask(self, sz):
         mask = (torch.triu(torch.ones(sz, sz)) == 1).transpose(0, 1)

@@ -9,6 +9,7 @@ BatchNorm batch statistics are not implemented.
 import torch
 from torch import nn
 
+from ...engine_base import EngineModule
 from ...melception_engine import FEATURES, MelceptionEngine
 
 
@@ -64,7 +65,7 @@ class _InceptionAux(nn.Module):
         self.fc = nn.Linear(768, num_classes)
 
 
-class Melception(nn.Module):
+class Melception(EngineModule):
     def __init__(self, num_classes, features_list, feature_extractor_weights_path, aux_logits=True, transform_input=False, dropout=0.5, **kwargs):
         """As the reference: Inception3(num_classes, aux_logits, ...) with a 1-channel Conv2d_1a_3x3, no max pools in the stem, weights loaded
         strictly from torch.load(path)['model'] and frozen.  transform_input and dropout have no effect on the reference's forward either."""
@@ -95,17 +96,10 @@ class Melception(nn.Module):
         self.Mixed_7c = _inception_e(2048)
         self.fc = nn.Linear(2048, num_classes)
         self.engine = MelceptionEngine(self)
-        self.register_load_state_dict_post_hook(lambda module, inc: module.engine.__setattr__("packed", False))
         state_dict = torch.load(feature_extractor_weights_path, map_location="cpu")
         self.load_state_dict(state_dict["model"])
         for p in self.parameters():
             p.requires_grad_(False)
-
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        if hasattr(self, "engine"):
-            self.engine.packed = False
-        return out
 
     @torch.no_grad()
     def forward(self, x):

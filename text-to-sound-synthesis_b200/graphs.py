@@ -1,7 +1,22 @@
-"""Tiny CUDA-graph cache: capture a fixed-shape launch sequence once, replay it with fresh inputs copied into static buffers."""
+"""CUDA-graph capture: one warm-up-then-capture sequence, and a tiny cache that replays a fixed-shape launch sequence with fresh inputs copied
+into static buffers."""
 from __future__ import annotations
 
 import torch
+
+
+def capture(step, device=None) -> torch.cuda.CUDAGraph:
+    """Run step() once on a side stream, then capture it: lazy initialisation (function attributes, weight packing, workspaces) happens in the
+    warm-up, so the captured launch sequence is the steady-state one.  The capture itself executes nothing."""
+    s = torch.cuda.Stream(device=device)
+    s.wait_stream(torch.cuda.current_stream(device))
+    with torch.cuda.stream(s):
+        step()
+    torch.cuda.current_stream(device).wait_stream(s)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        step()
+    return g
 
 
 class GraphCache:
@@ -16,15 +31,9 @@ class GraphCache:
         ent = self._entries.get(key)
         if ent is None:
             static_in = [t.clone() for t in inputs]
-            s = torch.cuda.Stream()
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):  # warm-up: lazy initialisation (function attributes, weight packing) must not be captured
-                fn(*static_in)
-            torch.cuda.current_stream().wait_stream(s)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                static_out = fn(*static_in)
-            ent = (g, static_in, static_out)
+            out = []
+            g = capture(lambda: out.append(fn(*static_in)))
+            ent = (g, static_in, out[-1])  # the captured call's outputs
             self._entries[key] = ent
         g, static_in, static_out = ent
         for dst, src in zip(static_in, inputs):

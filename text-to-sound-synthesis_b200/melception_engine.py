@@ -28,6 +28,7 @@ from __future__ import annotations
 import torch
 
 from . import ops
+from .engine_base import PackedEngine
 from .graphs import GraphCache
 from .packing import PackedConv, activation_scale
 
@@ -61,19 +62,15 @@ class _Act:
 
 
 
-class MelceptionEngine:
+class MelceptionEngine(PackedEngine):
+    settings = ("use_cuda_graph", "max_batch", "mean", "std")
+
     def __init__(self, module):
-        self.m = module
-        self.packed = False
+        super().__init__(module)
         self.use_cuda_graph = True
         self.max_batch = 64  # clips per pass: one 288-channel stage-A pair image is ~20 MB per clip at T = 848
         self._graphs = GraphCache()
         self.mean = self.std = None
-        self._param_sig = None
-
-    def _signature(self):
-        """(storage pointer, in-place version counter) of every parameter and BatchNorm buffer: changes on load_state_dict, .to(), p.data.copy_()."""
-        return tuple((t.data_ptr(), t._version) for t in self.m.state_dict(keep_vars=True).values())
 
     def set_normalization(self, mean=None, std=None):
         """Per-mel-bin (x - mean[f]) / std[f] fused into the stem (StandardNormalizeAudio, vggishish/transforms.py:13-40); None: inputs are
@@ -94,8 +91,7 @@ class MelceptionEngine:
         b = c.bn.bias.detach().double() - c.bn.running_mean.detach().double() * s
         return (w * s.view(-1, 1, 1, 1)).float(), b.float()
 
-    @torch.no_grad()
-    def repack(self):
+    def _pack(self):
         dev = self.m.fc.weight.device
         if dev.type != "cuda":
             raise RuntimeError("MelceptionEngine needs the module on a CUDA device (no CPU fallback)")
@@ -120,8 +116,6 @@ class MelceptionEngine:
             self._forward(x, 3, calibrate=True)
         finally:
             self.mean, self.std = mean, std
-        self.packed = True
-        self._param_sig = self._signature()
 
     # ------------------------------------------------------------------------------------------------ producers of one stored tensor
     def _produce(self, key, prods, calibrate, extra_amax=0.0):
@@ -335,8 +329,7 @@ class MelceptionEngine:
             raise ValueError(f"unknown Melception features {unknown}; choose from {FEATURES}")
         if x.dim() != 3:
             raise RuntimeError(f"Melception input must be (B, n_mels, T), got {tuple(x.shape)}")
-        if not self.packed or self._param_sig != self._signature():
-            self.repack()
+        self.ensure_current()
         x = x.detach().float().contiguous()
         depth = max(_DEPTH[f] for f in features)
         outs = []

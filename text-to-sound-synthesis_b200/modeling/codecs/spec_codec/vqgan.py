@@ -12,6 +12,7 @@ from torch import nn
 
 from ....decoder_engine import DecoderEngine
 from ....encoder_engine import EncoderEngine
+from ....engine_base import EngineModule
 
 
 class ColumnMajor(nn.Module):
@@ -172,7 +173,7 @@ class VectorQuantizer(nn.Module):
         return z
 
 
-class VQModel(nn.Module):
+class VQModel(EngineModule):
     def __init__(self, ddconfig, lossconfig=None, n_embed=256, embed_dim=256, ckpt_path=None, ignore_keys=[], image_key="image",
                  colorize_nlabels=None, monitor=None, precision="f16x3"):
         super().__init__()
@@ -185,11 +186,6 @@ class VQModel(nn.Module):
         self.post_quant_conv = nn.Conv2d(embed_dim, ddconfig["z_channels"], 1)
         self.engine = DecoderEngine(self, precision=precision)
         self.enc_engine = EncoderEngine(self)
-
-        def _stale(module, inc):
-            module.engine.packed = False
-            module.enc_engine.packed = False
-        self.register_load_state_dict_post_hook(_stale)
         if ckpt_path is not None:
             self.init_from_ckpt(ckpt_path, ignore_keys=ignore_keys)
 
@@ -200,14 +196,6 @@ class VQModel(nn.Module):
                 del sd[k]
         self.load_state_dict(sd, strict=False)  # encoder / loss keys are ignored, as with the reference's strict=False
         print(f"Restored from {path}")
-
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        if hasattr(self, "engine"):
-            self.engine.packed = False
-        if hasattr(self, "enc_engine"):
-            self.enc_engine.packed = False
-        return out
 
     @torch.no_grad()
     def encode(self, x):

@@ -11,6 +11,7 @@ import torch
 from torch import nn
 
 from ... import ops
+from ...engine_base import EngineModule
 from ...text_engine import TextTowerEngine
 
 _TEXT_CONFIGS = {"ViT-B/32": dict(width=512, layers=12, heads=8, ctx=77, embed=512), "ViT-B/16": dict(width=512, layers=12, heads=8, ctx=77, embed=512)}
@@ -40,7 +41,7 @@ class _Transformer(_Holder):
         self.resblocks = nn.Sequential(*[_ResBlock(width, heads) for _ in range(layers)])
 
 
-class CLIPTextEmbedding(nn.Module):
+class CLIPTextEmbedding(EngineModule):
     def __init__(self, clip_name="ViT-B/32", num_embed=49408, normalize=True, pick_last_embedding=True, keep_seq_len_dim=False,
                  additional_last_embedding=False, embed_dim=1024, clip_ckpt_path=None, text_layers=None):
         super().__init__()
@@ -62,7 +63,6 @@ class CLIPTextEmbedding(nn.Module):
             p.requires_grad = False
         self.eval()
         self.engine = TextTowerEngine(self)
-        self.register_load_state_dict_post_hook(lambda module, inc: module.engine.__setattr__("packed", False))
         if clip_ckpt_path is not None:
             self.load_clip_checkpoint(clip_ckpt_path)
 
@@ -91,12 +91,6 @@ class CLIPTextEmbedding(nn.Module):
     def train(self, mode=True):  # BaseEmbedding.train: a frozen embedding stays in eval mode
         self.training = mode and self.trainable
         return self
-
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        if hasattr(self, "engine"):
-            self.engine.packed = False
-        return out
 
     @property
     def dtype(self):

@@ -15,6 +15,7 @@ from torch import nn
 
 from ... import ops
 from ... import train_ops
+from ...graphs import capture
 from ...utils.misc import instantiate_from_config
 
 _SCHED_ROWS = ["log_at", "log_bt", "log_ct", "log_1_min_ct", "log_cumprod_at", "log_cumprod_bt", "log_cumprod_ct", "log_1_min_cumprod_ct"]
@@ -277,19 +278,10 @@ class DiffusionTransformer(nn.Module):
         gen = torch.cuda.default_generators[dev.index if dev.index is not None else torch.cuda.current_device()]
         seed, offset = gen.initial_seed(), gen.get_offset()
         nthreads, counter_offset = ops.aten_rand_geometry(B * (K + 1) * L, dev)
-        if self.use_cuda_graph and st["graph"] is None:
-            # warm-up on a side stream (lazy inits: cudaFuncSetAttribute, workspaces), then capture one step; the loop state is re-armed afterwards
+        if self.use_cuda_graph and st["graph"] is None:  # the warm-up runs one step: the loop state is re-armed afterwards
             self._arm_loop(st, steps, post_steps, seed, offset, counter_offset, nthreads)
             st["x"].fill_(K)
-            s = torch.cuda.Stream(device=dev)
-            s.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(s):
-                self._fused_step(st)
-            torch.cuda.current_stream(dev).wait_stream(s)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._fused_step(st)
-            st["graph"] = g
+            st["graph"] = capture(lambda: self._fused_step(st), dev)
             self._graphs[key] = st
         self._arm_loop(st, steps, post_steps, seed, offset, counter_offset, nthreads)
         if x_init is None:

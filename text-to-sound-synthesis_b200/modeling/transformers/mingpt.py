@@ -16,6 +16,7 @@ from torch import nn
 
 from ... import ops
 from ...ar_engine import AREngine, check_ar_shapes
+from ...engine_base import EngineModule
 from ...utils.misc import instantiate_from_config
 
 
@@ -73,7 +74,7 @@ class Block(nn.Module):
         raise RuntimeError("Block only stores parameters; compute runs in AREngine (CUDA kernels)")
 
 
-class GPT(nn.Module):
+class GPT(EngineModule):
     """mingpt.py:141-187: tok_emb, pos_emb (1, block_size, D), blocks, ln_f, head (no bias)."""
 
     def __init__(self, vocab_size, block_size, n_layer=12, n_head=8, n_embd=256, embd_pdrop=0., resid_pdrop=0., attn_pdrop=0., n_unmasked=0):
@@ -102,12 +103,6 @@ class GPT(nn.Module):
         elif isinstance(module, nn.LayerNorm):
             module.bias.data.zero_()
             module.weight.data.fill_(1.0)
-
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        if hasattr(self, "engine"):
-            self.engine.packed = False
-        return out
 
     def _check(self, n_pos: int) -> None:
         """Refusals, before anything is launched: kernel limits, then the reference's block-size assert (mingpt.py:170)."""

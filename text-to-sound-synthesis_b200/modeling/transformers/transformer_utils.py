@@ -5,13 +5,13 @@ Same constructor arguments and the same state_dict keys (SURVEY.md section 8b), 
 training goes through ``DenoiserTrainEngine`` (called from DiffusionTransformer._train_loss).  The sub-modules
 below only HOLD parameters under the reference's names -- they have no torch forward (there is no fallback path).
 """
-import copy
 import math
 
 import torch
 from torch import nn
 
 from ...engine import DenoiserEngine
+from ...engine_base import EngineModule
 from ...train_engine import DenoiserTrainEngine
 from ...utils.misc import instantiate_from_config
 
@@ -69,7 +69,7 @@ class Block(_ParamOnly):
         self.mlp = nn.Sequential(nn.Linear(n_embd, mlp_hidden_times * n_embd), GELU2(), nn.Linear(mlp_hidden_times * n_embd, n_embd), nn.Dropout(0.0))
 
 
-class Text2ImageTransformer(nn.Module):
+class Text2ImageTransformer(EngineModule):
     def __init__(self, condition_seq_len=77, n_layer=14, n_embd=1024, n_head=16, content_seq_len=1024, attn_pdrop=0, resid_pdrop=0,
                  mlp_hidden_times=4, block_activate=None, attn_type="selfcross", content_spatial_size=[32, 32], condition_dim=512,
                  diffusion_step=1000, timestep_type="adalayernorm", content_emb_config=None, mlp_type="fc", checkpoint=False,
@@ -95,21 +95,6 @@ class Text2ImageTransformer(nn.Module):
         self.apply(self._init_weights)
         self.engine = DenoiserEngine(self, precision=precision)
         self.train_engine = DenoiserTrainEngine(self, precision=train_precision)  # forward-with-activations + backward (A13)
-        self.register_load_state_dict_post_hook(lambda module, incompatible: module.engine.__setattr__("packed", False))
-
-    def __deepcopy__(self, memo):
-        """EMA's copy.deepcopy (reference engine/ema.py:19): copy parameters / buffers / hooks, give the copy its own fresh engines (packed weights,
-        workspaces with saved activations and captured CUDA graphs are caches of THIS instance and cannot be deep-copied)."""
-        cls = self.__class__
-        new = cls.__new__(cls)
-        memo[id(self)] = new
-        for k, v in self.__dict__.items():
-            if k in ("engine", "train_engine"):
-                continue
-            new.__dict__[k] = copy.deepcopy(v, memo)
-        new.engine = DenoiserEngine(new, precision=self.engine.precision)
-        new.train_engine = DenoiserTrainEngine(new, precision=self.train_engine.precision)
-        return new
 
     def _init_weights(self, module):  # same distribution as the reference (:355-363)
         if isinstance(module, (nn.Linear, nn.Embedding)):
@@ -120,10 +105,8 @@ class Text2ImageTransformer(nn.Module):
             module.bias.data.zero_()
             module.weight.data.fill_(1.0)
 
-    def _apply(self, fn, *a, **k):  # .cuda()/.to(): packed copies go stale
+    def _apply(self, fn, *a, **k):  # .cuda() / .to(): the training engine's operands and workspaces go stale too
         out = super()._apply(fn, *a, **k)
-        if hasattr(self, "engine"):
-            self.engine.packed = False
         if hasattr(self, "train_engine"):
             self.train_engine.reset()
         return out

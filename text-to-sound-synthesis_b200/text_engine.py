@@ -12,16 +12,15 @@ import math
 import torch
 
 from . import ops
+from .engine_base import PackedEngine
 
 
-class TextTowerEngine:
+class TextTowerEngine(PackedEngine):
     def __init__(self, module):
-        self.m = module
-        self.packed = False
+        super().__init__(module)
         self.launches = 0
 
-    @torch.no_grad()
-    def repack(self):
+    def _pack(self):
         m = self.m
         dev = m.token_embedding.weight.device
         if dev.type != "cuda":
@@ -41,13 +40,11 @@ class TextTowerEngine:
                 wo=h(blk.attn.out_proj.weight), bo=f(blk.attn.out_proj.bias), g2=f(blk.ln_2.weight), b2=f(blk.ln_2.bias), e2=blk.ln_2.eps,
                 wfc=h(blk.mlp.c_fc.weight), bfc=f(blk.mlp.c_fc.bias), wpr=h(blk.mlp.c_proj.weight), bpr=f(blk.mlp.c_proj.bias)))
         self.gf, self.bf, self.ef = f(m.ln_final.weight), f(m.ln_final.bias), m.ln_final.eps
-        self.packed = True
 
     @torch.no_grad()
     def forward(self, tokens: torch.Tensor, normalize: bool = True) -> torch.Tensor:
         """tokens (B, L) int64 (negative = padding, read as id 0 like the reference's in-place clamp) -> (B, L, D) fp32."""
-        if not self.packed:
-            self.repack()
+        self.ensure_current()
         B, L = tokens.shape
         D, H = self.D, self.H
         if L > self.pos.shape[0]:

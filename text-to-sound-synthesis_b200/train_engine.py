@@ -48,6 +48,9 @@ class DenoiserTrainEngine:
         self._kernel_device = "cuda"  # the kernels exist for CUDA only; tests/test_cpu_train_engine.py swaps in CPU stand-ins to check the orchestration
         self.forward_id = 0         # activations live in engine-owned buffers: backward() must follow ITS forward (checked by the caller)
 
+    def __deepcopy__(self, memo):  # a deep copy of the module gets a fresh engine: operands, workspaces and graphs are per-instance caches
+        return DenoiserTrainEngine(memo.get(id(self.m), self.m), precision=self.precision)
+
     # ------------------------------------------------------------------ small helpers
     @property
     def device(self):

@@ -6,6 +6,7 @@ import numpy as np
 import torch
 from torch import nn
 
+from ..engine_base import EngineModule
 from ..vocoder_engine import VocoderEngine
 
 
@@ -27,7 +28,7 @@ class ResnetBlock(_Holder):
         self.shortcut = _wn(nn.Conv1d(dim, dim, kernel_size=1))
 
 
-class Generator(nn.Module):
+class Generator(EngineModule):
     def __init__(self, input_size, ngf, n_residual_layers, precision="f16x3"):
         super().__init__()
         ratios = [8, 8, 2, 2]
@@ -48,13 +49,6 @@ class Generator(nn.Module):
             if isinstance(m, (nn.Conv1d, nn.ConvTranspose1d)):
                 m.weight_v.data.normal_(0.0, 0.02)
         self.engine = VocoderEngine(self, precision=precision)
-        self.register_load_state_dict_post_hook(lambda module, inc: module.engine.__setattr__("packed", False))
-
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        if hasattr(self, "engine"):
-            self.engine.packed = False
-        return out
 
     @torch.no_grad()
     def forward(self, x):

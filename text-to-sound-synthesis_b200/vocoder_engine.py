@@ -30,6 +30,7 @@ from __future__ import annotations
 import torch
 
 from . import ops
+from .engine_base import PackedEngine
 from .graphs import GraphCache
 from .packing import PackedConv as _PackedConv, activation_scale
 
@@ -46,29 +47,29 @@ def _fold(m) -> torch.Tensor:
     return g * v / v.flatten(1).norm(dim=1).view(-1, *([1] * (v.dim() - 1)))
 
 
-class VocoderEngine:
+class VocoderEngine(PackedEngine):
+    settings = ("use_cuda_graph", "max_batch")
+
     def __init__(self, gen, precision: str = "f16x3"):
         if precision != "f16x3":
             raise ValueError("the MelGAN engine computes in split-fp16 ('f16x3': fp32-class accuracy on the fp16 tensor pipe)")
-        self.gen = gen
+        super().__init__(gen, precision=precision)
         self.precision = precision
-        self.packed = False
         self.launches = 0
         self.use_cuda_graph = True
         self.max_batch = 32  # clips per pass (8 bytes per activation element: 55.6 MB per clip for the widest stage)
         self._graphs = GraphCache()
         self._bufs = {}
 
-    @torch.no_grad()
-    def repack(self):
-        mods = list(self.gen.model)
+    def _pack(self):
+        mods = list(self.m.model)
         dev = mods[1].bias.device
         w0 = _fold(mods[1])  # (16*ngf, n_mel, 7)
         self.n_mel = w0.shape[1]
         self.first = _PackedConv([w0[:, :, j] for j in range(w0.shape[2])], mods[1].bias)
         self.stages = []
         i = 2
-        for r in self.gen.ratios:
+        for r in self.m.ratios:
             ct = mods[i + 1]
             w = _fold(ct)  # (Cin, Cout, 2r); weight_norm dim=0 -> norm over (Cout, k) per input channel
             p = r // 2 + r % 2
@@ -83,7 +84,7 @@ class VocoderEngine:
             st = dict(r=r, cin=w.shape[0], cout=cout, half=half, ca=_PackedConv(wa, ct.bias.detach().repeat(half)),
                       cb=_PackedConv(wb, ct.bias.detach().repeat(r - half)), res=[])
             i += 2
-            for _ in range(self.gen.n_residual_layers):
+            for _ in range(self.m.n_residual_layers):
                 rb = mods[i]
                 wd, w1, ws = _fold(rb.block[2]), _fold(rb.block[4]), _fold(rb.shortcut)
                 # g2 (shortcut | 1x1) is packed during calibration: its 1x1 half absorbs the ratio of the two operands' activation scales
@@ -112,7 +113,6 @@ class VocoderEngine:
         for st in self.stages:
             for rb in st["res"]:
                 rb.pop("ws"), rb.pop("w1")
-        self.packed = True
 
     def _buffers(self, B, T0, dev):
         key = (B, T0)
@@ -129,10 +129,9 @@ class VocoderEngine:
 
     @torch.no_grad()
     def forward(self, mel: torch.Tensor) -> torch.Tensor:
-        if not mel.is_cuda or list(self.gen.model)[1].bias.device.type != "cuda":
+        if not mel.is_cuda or list(self.m.model)[1].bias.device.type != "cuda":
             raise RuntimeError("VocoderEngine.forward needs the module and its input on a CUDA device (no CPU fallback)")
-        if not self.packed:
-            self.repack()
+        self.ensure_current()
         mel = mel.detach().float().contiguous()
         if mel.shape[0] > self.max_batch:
             return torch.cat([self.forward(mel[i:i + self.max_batch]) for i in range(0, mel.shape[0], self.max_batch)], 0)
